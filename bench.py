@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- calibration / fake-quant throughput of the PPQ quantization-simulation hot path on B200.
+"""bench.py -- calibration / fake-quant throughput of the PPQ quantization-simulation hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--workload resnet50|yolov5s] [--impl ours|reference]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): ResNet-50 RuntimeCalibrationPass, minmax + KL-histogram, 512 synthetic 3x224x224 samples per GPU,
@@ -41,7 +42,8 @@ METRIC = 'calibration_imgs_per_s'
 UNIT = 'imgs/s'
 BINS = 4096
 SAMPLES_PER_GPU = 512
-VENDOR_HBM_GBS = 8000.0          # NVIDIA's B200 HBM3e figure (BASELINE.md §3 asks for both denominators)
+VENDOR_HBM_GBS = 3350.0          # NVIDIA's H100 SXM data-sheet HBM3 bandwidth: a denominator, not a measured peak
+DUMP_SAMPLE = 1 << 22            # fake-quantised weight elements written by --dump-outputs (16 MB of float32)
 
 
 # ------------------------------------------------------------------------------------------------ workload definition
@@ -219,13 +221,7 @@ class ClockSampler(threading.Thread):
 
 
 def measured_peaks():
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs: device-to-device copy, read + write)'
-        except Exception:
-            pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return VENDOR_HBM_GBS, 'NVIDIA H100 SXM data sheet (3.35 TB/s HBM3)'
 
 
 def stats(v):
@@ -247,13 +243,14 @@ def run_ours(args, rank, world, local_rank):
     stream = torch.cuda.current_stream()
     hist_events, mm_events, launches = [], [], [0]
     wq = MultiWeightQuantizer(wl.w, wl.w_scale, wl.w_offset, channel_axis=0)
+    fake_quant_weights = [None]                                   # what the last weight pass returned
 
     def weights_pass():
         if args.per_tensor_weight_launches:
-            for w, s, o in zip(wl.w, wl.w_scale, wl.w_offset): ext.QuantizeTensor_LC(w, s, o, -128, 127, 0, 0)
+            fake_quant_weights[0] = [ext.QuantizeTensor_LC(w, s, o, -128, 127, 0, 0) for w, s, o in zip(wl.w, wl.w_scale, wl.w_offset)]
             launches[0] += len(wl.w)
         else:
-            wq()                                                  # all weights, one launch
+            fake_quant_weights[0] = wq()                          # all weights, one launch
             launches[0] += 1
 
     def calibrate(timed):
@@ -314,6 +311,8 @@ def run_ours(args, rank, world, local_rank):
         per_rank = [torch.zeros_like(mine) for _ in range(world)]
         dist.all_gather(per_rank, mine)
     assert torch.isfinite(scales).all() and (scales > 0).all()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, cal, fake_quant_weights[0])
 
     # ---- roofline of the dominant kernel (multi-tensor histogram; 4 B/element) from the events of the timed region
     peak, peak_src = measured_peaks()
@@ -321,14 +320,8 @@ def run_ours(args, rank, world, local_rank):
     m_ms = sum(m_list) / len(m_list)
     hist_gbs = 4.0 * wl.act_elems / (h_ms * 1e-3) / 1e9
     mm_gbs = 4.0 * wl.act_elems / (m_ms * 1e-3) / 1e9
-    traffic = None
-    try:                                                                    # dram__bytes_read + dram__bytes_write of one launch, from the committed ncu capture
-        tj = json.load(open(os.path.join(ROOT, 'profiles', 'r02_traffic.json')))
-        if tj.get('batch') == args.batch and args.workload == 'resnet50': traffic = tj['traffic_bytes_per_launch']
-    except Exception:
-        pass
     roofline = {'bound': 'hbm', 'kernel': 'multi_histogram_t_kernel', 'achieved': round(hist_gbs, 1), 'peak': peak, 'unit': 'GB/s',
-                'frac': round(hist_gbs / peak, 4), 'traffic': traffic, 'peak_source': peak_src,
+                'frac': round(hist_gbs / peak, 4), 'peak_source': peak_src,
                 'peak_vendor': VENDOR_HBM_GBS, 'frac_of_vendor_peak': round(hist_gbs / VENDOR_HBM_GBS, 4), 'ms_per_launch': round(h_ms, 4),
                 'algorithmic_bytes_per_launch': 4 * wl.act_elems,
                 'other_kernels': {'multi_minmax_t_kernel': {'achieved': round(mm_gbs, 1), 'frac': round(mm_gbs / peak, 4),
@@ -366,6 +359,20 @@ def run_ours(args, rank, world, local_rank):
     if rank == 0:
         result['cpu_baseline'] = cpu_baseline(args) if not args.no_cpu_baseline else None
     return result
+
+
+def dump_outputs(out_dir, cal, weights):
+    """What the last timed step handed back to its caller: the per-tensor scale and offset of the calibration and a fixed, seeded sample of
+    the fake-quantised weights (all of them would be 102 MB for ResNet-50), each as <out_dir>/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = torch.cat([w.reshape(-1) for w in weights])
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+    arrays = {'calibration_scale': cal.scale, 'calibration_offset': cal.offset,
+              'weights_fake_quant_sample': flat[idx.to(flat.device)]}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a.detach().cpu().numpy())
 
 
 def fakequant_sweep(ext, device, peak):
@@ -566,7 +573,7 @@ def run_reference(args, rank, world):
 
 
 def host_cpu_quota():
-    """CPUs this process may actually use (cgroup quota / affinity), not the CPUs the host reports: the B200 boxes report 128 and grant 16, and
+    """CPUs this process may actually use (cgroup quota / affinity), not the CPUs the host reports: a shared host may report 128 and grant 16, and
     one OpenMP thread per *reported* CPU makes torch's host-side ops crawl (spinning threads under a CFS quota)."""
     n = os.cpu_count() or 1
     try: n = min(n, len(os.sched_getaffinity(0)))
@@ -595,12 +602,14 @@ def main():
     ap.add_argument('--rotate', type=int, default=4, help='distinct activation sets cycled through (each > L2)')
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--e2e-steps', type=int, default=5, help='timed end-to-end calibrations of 512 samples (each ~0.12 s)')
-    ap.add_argument('--e2e-nchw', action='store_true', help='run the torch network of the e2e arm in NCHW; default is NHWC (channels_last: cuDNN\'s native layout -- '
-                    'measured 3.09 vs 3.83-4.24 ms per 32-image forward; the hot path reads dense tensors in storage order either way)')
+    ap.add_argument('--e2e-nchw', action='store_true', help='run the torch network of the e2e arm in NCHW; default is NHWC (channels_last: cuDNN\'s native layout; '
+                    'the hot path reads dense tensors in storage order either way)')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-sweep', action='store_true')
     ap.add_argument('--no-cpu-baseline', action='store_true', help='profiling runs only')
     ap.add_argument('--ref-budget', type=float, default=100.0, help='wall-clock budget (s) of the CPU reference arm')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last step computed (scales, offsets, a seeded sample of the fake-quantised weights) as DIR/<name>.npy')
     ap.add_argument('--per-tensor-weight-launches', action='store_true', help='one QuantizeTensor_LC launch per weight (the reference flow) instead of the multi-tensor launch')
     args = ap.parse_args()
     if args.batch is None: args.batch = WORKLOADS[args.workload]['batch']

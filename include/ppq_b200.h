@@ -1,5 +1,5 @@
 /*
- * ppq_b200.h -- C ABI of libppq_b200.so: B200 (sm_100a) kernels for the PPQ quantization-simulation hot path.
+ * ppq_b200.h -- C ABI of libppq_b200.so: H100 (sm_90a) kernels for the PPQ quantization-simulation hot path.
  *
  * This is the drop-in boundary.  Every entry point replaces one function of the reference's native extension
  * `PPQ_Cuda_Impls` (pybind table: /root/reference/ppq/csrc/export.cc:8-34, bound by ppq/core/ffi.py:56-350);
@@ -39,7 +39,7 @@ extern "C" {
 /* ---- library ----------------------------------------------------------------------------------- */
 PPQ_B200_API int         ppq_b200_abi_version(void);              /* bumps when a signature changes */
 PPQ_B200_API const char *ppq_b200_error_string(int status);
-PPQ_B200_API const char *ppq_b200_build_info(void);               /* "sm_100a nvcc 12.9 ..." */
+PPQ_B200_API const char *ppq_b200_build_info(void);               /* "sm_90a nvcc 12.9 ..." */
 /* Runtime tuning knob used by bench/profiling to select a kernel variant (0 = default). */
 PPQ_B200_API int         ppq_b200_set_variant(const char *kernel, int variant);
 PPQ_B200_API int         ppq_b200_get_variant(const char *kernel);
@@ -148,7 +148,7 @@ PPQ_B200_API int ppq_b200_quantile_t_guess(const float *x, int64_t n, float q, f
 /* replaces Isotone_T, sort.cu:23-40, 61-73: out4 = {sorted[n-1], sorted[n-2], sorted[0], sorted[1]} (same workspace). */
 PPQ_B200_API int ppq_b200_isotone_t(const float *x, int64_t n, float *out4, void *workspace, void *stream);
 
-/* ---- multi-tensor collectors (one launch over a table of tensors; the B200-native calibration path) ---------
+/* ---- multi-tensor collectors (one launch over a table of tensors; the H100-native calibration path) ---------
  * A descriptor lives in DEVICE memory.  `slot` selects the statistics slot in the arena:
  *   minmax arena: float[2 * slots]  ({min, max} per slot);   hist arena: int32[slots * bins];
  *   hist_scale arena: float[slots]. */

@@ -19,8 +19,8 @@ Pinning status (tests/test_oracle_pinning.py):
   KL search, KL divergence: pinned against tests/golden/ (generated from the real reference, CPU path).
   compute_mse_loss: pinned against the reference's own hist_mse.cc (oracle/_ref/hist_mse_ref.so + fixture).
   FP8 (QuantizeTensor_FT/_FC), Histogram_T/_Asymmetric_T/_C device semantics, Quantile_T:
-  the reference has no CPU implementation and no test -> pinned on the B200 box against the reference's own
-  CUDA kernels compiled for sm_100a (oracle/_ref/PPQ_Cuda_Impls_ref.so, tests/test_gpu_vs_reference_cuda.py);
+  the reference has no CPU implementation and no test -> pinned on the GPU against the reference's own
+  CUDA kernels compiled for sm_90a (oracle/_ref/PPQ_Cuda_Impls_ref.so, tests/test_gpu_vs_reference_cuda.py);
   fixtures produced there are committed under tests/golden/ref_cuda_*.npz once available.
 """
 import ctypes
@@ -40,7 +40,7 @@ RND_HALF_FAR_FROM_ZERO, RND_TO_NEAR_INT, RND_UP, RND_DOWN = 4, 5, 6, 7
 
 def host_threads() -> int:
     """CPU threads this process may really use: the scheduler affinity mask capped by the cgroup CPU quota.  os.cpu_count() reports
-    the whole host (128 on the B200 boxes) even when the container is limited to a few cores; running torch CPU ops with one thread
+    the whole host (128 on some shared GPU hosts) even when a CPU quota limits the process to a few cores; running torch CPU ops with one thread
     per *host* core then oversubscribes the quota by an order of magnitude."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, 'sched_getaffinity') else (os.cpu_count() or 1)
     for path in ('/sys/fs/cgroup/cpu.max', '/sys/fs/cgroup/cpu/cpu.cfs_quota_us'):

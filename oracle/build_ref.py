@@ -9,9 +9,9 @@ Two artefacts:
   oracle/_ref/PPQ_Cuda_Impls_ref*.so
                                    the reference's own torch extension (export.cc + cuda/{linear,sort,train,
                                    floating}.cu + cpu/hist_mse.cc: exactly the source list of
-                                   ppq/core/ffi.py:31-38) compiled for sm_100a with this image's nvcc/torch.
-                                   On the B200 box it is the GPU-side oracle (bit-parity for FP8, which has no
-                                   CPU path in the reference) and the competitor kernel we time ours against.
+                                   ppq/core/ffi.py:31-38) compiled for sm_90a with the local nvcc/torch.
+                                   With PPQ_RECORD_REFERENCE set, the GPU tests call it and record what it returns
+                                   (tests/refcuda.py, tests/golden/ref_cuda_calls.json.gz).
 
 We do NOT run the reference's build system (its JIT writes into the read-only package dir); the
 compile lines are ours (torch.utils.cpp_extension.load pointed at a writable build dir).
@@ -51,7 +51,7 @@ def build_cuda_ext(force: bool = False) -> str:
     so = os.path.join(OUT, 'PPQ_Cuda_Impls_ref.so')
     if os.path.exists(so) and not force:
         return so
-    os.environ['TORCH_CUDA_ARCH_LIST'] = '10.0a'
+    os.environ['TORCH_CUDA_ARCH_LIST'] = '9.0a'
     os.environ.setdefault('MAX_JOBS', '6')
     from torch.utils.cpp_extension import load
     load(name='PPQ_Cuda_Impls_ref',
@@ -63,7 +63,7 @@ def build_cuda_ext(force: bool = False) -> str:
                   os.path.join(CSRC, 'cpu', 'hist_mse.cc')],
          build_directory=OUT, with_cuda=True, extra_cflags=['-O3'],
          extra_cuda_cflags=['-lineinfo'], is_python_module=False, verbose=True)
-    # drop the object files (64 MiB gpurun_out limit does not apply to the snapshot, but keep it lean)
+    # drop the object files: only the shared object is used
     for f in os.listdir(OUT):
         if f.endswith('.o'):
             os.remove(os.path.join(OUT, f))

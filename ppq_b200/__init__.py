@@ -1,4 +1,4 @@
-"""ppq_b200 -- B200-native (sm_100a) implementation of the PPQ quantization-simulation hot path.
+"""ppq_b200 -- H100-native (sm_90a) implementation of the PPQ quantization-simulation hot path.
 
     csrc/        hand-written CUDA kernels + C ABI (include/ppq_b200.h) + torch binding with the reference's 20 names
     ffi          mirror of ppq.core.ffi  (CUDA_COMPLIER, class CUDA)

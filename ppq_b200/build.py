@@ -2,11 +2,11 @@
 
     python -m ppq_b200.build [--force] [--no-torch]
 
-  ppq_b200/_lib/libppq_b200.so   C-ABI library (include/ppq_b200.h): hand-written sm_100a kernels, CUDA runtime only.
+  ppq_b200/_lib/libppq_b200.so   C-ABI library (include/ppq_b200.h): hand-written sm_90a kernels, CUDA runtime only.
   ppq_b200/_C.so                 torch/pybind layer exporting the reference's 20 names (csrc/torch_binding.cc).
 
-nvcc cross-compiles for sm_100a without a GPU.  Flags of record:
-  -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -fmad=false
+nvcc cross-compiles for sm_90a without a GPU.  Flags of record:
+  -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false
 (-fmad=false: every fused multiply-add in the kernels is written explicitly with __fmaf_rn; nothing else may contract,
  which is part of the bit-exactness contract with the reference.)
 """
@@ -26,7 +26,7 @@ EXT = os.path.join(HERE, '_C.so')
 INCLUDE = os.path.join(os.path.dirname(HERE), 'include')
 
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-fmad=false',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-fmad=false',
               '--expt-relaxed-constexpr', '--expt-extended-lambda',
               '-Xcompiler', '-fPIC,-fvisibility=hidden,-ffp-contract=off,-Wall', '-I', INCLUDE]
 CU_SOURCES = ['fakequant.cu', 'fakequant_tma.cu', 'collectors.cu', 'search.cu', 'select.cu', 'train.cu', 'host.cc']
@@ -71,8 +71,8 @@ def build_lib(force=False, verbose=False):
                 if verbose and out.strip():
                     print(out)
     if jobs or force or not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(o) for o in objs):
-        # link under a temporary name, then rename: a snapshot of the tree (gpurun) never sees a half-written library
-        run([NVCC, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', LIB + '.tmp'] + objs + ['-cudart', 'shared', '-Xlinker', '--no-undefined'])
+        # link under a temporary name, then rename: a copy of the tree taken meanwhile never sees a half-written library
+        run([NVCC, '-gencode', 'arch=compute_90a,code=sm_90a', '-shared', '-o', LIB + '.tmp'] + objs + ['-cudart', 'shared', '-Xlinker', '--no-undefined'])
         os.replace(LIB + '.tmp', LIB)
     return LIB
 

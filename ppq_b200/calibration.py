@@ -1,7 +1,7 @@
 """Calibration drivers: the mirror of RuntimeCalibrationPass (/root/reference/ppq/quantization/optim/calibration.py:19-213)
 re-designed around a device-resident statistics arena and sample-sharded data parallelism (SURVEY.md §8e).
 
-  ArenaCalibrator          the B200-native two-phase calibrator.  All T observed tensors of one forward are collected by ONE
+  ArenaCalibrator          the H100-native two-phase calibrator.  All T observed tensors of one forward are collected by ONE
                            multi-tensor launch per phase (Multi_MinMax_T / Multi_Histogram_T) into one contiguous arena:
                                minmax [T,2] fp32,  hist_scale [T] fp32,  hist [T,bins] int32.
                            Rank r of R processes sees samples r, r+R, ...; the whole multi-GPU exchange is

@@ -1,4 +1,4 @@
-// collectors.cu -- sm_100a calibration collectors behind the C ABI of include/ppq_b200.h.
+// collectors.cu -- sm_90a calibration collectors behind the C ABI of include/ppq_b200.h.
 //
 //   ppq_b200_minmax_t / _c          fused single-pass min+max; replaces the two torch reductions of
 //                                   TorchMinMaxObserver.observe (/root/reference/ppq/quantization/observer/range.py:85-100)

@@ -1,4 +1,4 @@
-// common.cuh -- device helpers shared by the sm_100a kernels of libppq_b200.
+// common.cuh -- device helpers shared by the sm_90a kernels of libppq_b200.
 //
 // Numerics contract (restated in DESIGN.md, proven against oracle/ and the reference's own CUDA build):
 //   round2int<mode>   == _round2int            (/root/reference/ppq/csrc/cuda/common.cuh:88-114)
@@ -10,14 +10,14 @@
 
 namespace ppqb {
 
-// SM count of the CURRENT device (B200: 148 = 2 dies x 74), queried once per device ordinal; every persistent grid is sized from it.
+// SM count of the CURRENT device (H100 SXM: 132), queried once per device ordinal; every persistent grid is sized from it.
 inline int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     int v = cached[dev];
     if (v == 0) {
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         cached[dev] = v;
     }
     return v;
@@ -71,7 +71,7 @@ __device__ __forceinline__ int round2int_dyn(float v, int mode) {
 __device__ __forceinline__ int offset_to_int(float o) { return __float2int_rz(roundf(o)); }
 
 // ---- exact fp32 division by a (warp-)uniform divisor ------------------------------------------------------
-// x / s must be the correctly rounded IEEE quotient.  div.rn.f32 costs ~30 issue slots per element on sm_100a
+// x / s must be the correctly rounded IEEE quotient.  div.rn.f32 costs ~30 issue slots per element on sm_90a
 // (MUFU.RCP + 6 FFMA + FCHK + guarded slow-path call, measured from SASS), which would make an 8 B/element
 // streaming kernel issue-bound at HBM3e speed.  The divisor is constant per tensor (or per channel row), so we
 // hoist r = RN(1/s) and run Markstein's correction twice per element (1 FMUL + 4 FFMA):
@@ -143,7 +143,7 @@ __device__ __forceinline__ float4 exact_div4x(const ExactDiv &a, const ExactDiv 
 
 // ---- streaming global memory access -----------------------------------------------------------------------
 // Inputs are read exactly once: bypass L1 allocation (ld.global.nc.L1::no_allocate).  Outputs are written with
-// the default policy so that they stay in the 126 MB L2 for the consumer kernel (the next operator of the graph).
+// the default policy so that they stay in the 50 MB L2 for the consumer kernel (the next operator of the graph).
 __device__ __forceinline__ float4 ld_stream4(const float4 *p) {
     float4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"

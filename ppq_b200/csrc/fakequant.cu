@@ -1,4 +1,4 @@
-// fakequant.cu -- sm_100a fake-quant kernels (quantize -> clamp -> dequantize) behind the C ABI of include/ppq_b200.h.
+// fakequant.cu -- sm_90a fake-quant kernels (quantize -> clamp -> dequantize) behind the C ABI of include/ppq_b200.h.
 //
 //   ppq_b200_linear_quant_t / _c   replace QuantizeTensor_LT / _LC  (/root/reference/ppq/csrc/cuda/linear.cu:38-233)
 //   ppq_b200_float_quant_t  / _c   replace QuantizeTensor_FT / _FC  (ppq/csrc/cuda/floating.cu:36-131, common.cuh:154-226)
@@ -6,7 +6,7 @@
 //
 // Design (DESIGN.md §kernels): pure streaming kernels, 8 B/element of algorithmic HBM traffic (4 read + 4 write),
 // no reuse -> no shared-memory staging in the default variant.  Each thread keeps 4 independent 128-bit loads in flight
-// (64 B), 256 threads per CTA, persistent grid of 148 SMs x 8 CTAs, grid-stride over float4 vectors, so ~128 KB are in
+// (64 B), 256 threads per CTA, persistent grid of (SM count) x 8 CTAs, grid-stride over float4 vectors, so ~128 KB are in
 // flight per SM -- enough to cover HBM3e latency x bandwidth.  The arithmetic per element is kept under ~15 issue slots
 // (hoisted exact reciprocal + 2 Markstein corrections instead of div.rn, see common.cuh) so the kernel stays
 // bandwidth-bound rather than issue-bound.  Variant 1 (ppq_b200_set_variant("linear_quant_t", 1)) is the
@@ -496,7 +496,7 @@ static int launch_tensor(const float *x, OutT *y, int64_t n, const float *scale,
         ew_tensor_kernel<Op, OutT, true, 8><<<grid_for((n + 3) / 4, kThreads, 8, 16), kThreads, 0, st>>>(x, y, n, scale, offset, p);
         return (int)cudaGetLastError();
     }
-    const int grid = grid_for(vec ? (n + 3) / 4 : n, kThreads, vec ? kUnroll : 4, 8);       // persistent: 148 SMs x 8 CTAs
+    const int grid = grid_for(vec ? (n + 3) / 4 : n, kThreads, vec ? kUnroll : 4, 8);       // persistent: SM count x 8 CTAs
     if (vec) ew_tensor_kernel<Op, OutT, true><<<grid, kThreads, 0, st>>>(x, y, n, scale, offset, p);
     else     ew_tensor_kernel<Op, OutT, false><<<grid, kThreads, 0, st>>>(x, y, n, scale, offset, p);
     return (int)cudaGetLastError();

@@ -33,7 +33,7 @@ const char *ppq_b200_error_string(int status) {
 }
 
 const char *ppq_b200_build_info(void) {
-    return "libppq_b200 abi 1; sm_100a; host compiler gcc " __VERSION__ "; built " __DATE__;
+    return "libppq_b200 abi 1; sm_90a; host compiler gcc " __VERSION__ "; built " __DATE__;
 }
 
 int ppq_b200_set_variant(const char *kernel, int variant) {

@@ -1,4 +1,4 @@
-// search.cu -- scale / offset search on the device (sm_100a), behind the C ABI of include/ppq_b200.h.
+// search.cu -- scale / offset search on the device (sm_90a), behind the C ABI of include/ppq_b200.h.
 //
 //   ppq_b200_minmax_to_scale_offset   replaces minmax_to_scale_offset   (/root/reference/ppq/quantization/observer/range.py:22-75)
 //   ppq_b200_hist_scale_from_minmax   replaces the phase-1 render of TorchHistObserver (range.py:291-301)

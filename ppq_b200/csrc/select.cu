@@ -1,4 +1,4 @@
-// select.cu -- exact order statistics without sorting (sm_100a), behind the C ABI of include/ppq_b200.h.
+// select.cu -- exact order statistics without sorting (sm_90a), behind the C ABI of include/ppq_b200.h.
 //
 //   ppq_b200_quantile_t         replaces Quantile_T (/root/reference/ppq/csrc/cuda/sort.cu:6-20, 42-59): the reference clones the
 //                               tensor, thrust::sort's the clone and reads sorted[clip(rn(n*q))] and sorted[clip(rn(n*(1-q)))].

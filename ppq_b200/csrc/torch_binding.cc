@@ -9,7 +9,7 @@
 // epc computed from the trailing sizes instead of stride(channel_axis) (safe for size-1 dims), and a loud error
 // for CPU tensors instead of a crash.
 //
-// Extra names (not in the reference table) expose the B200-native calibration path: fused min/max, device-resident
+// Extra names (not in the reference table) expose the H100-native calibration path: fused min/max, device-resident
 // hist_scale, multi-tensor collectors and the on-device scale search.  ppq_b200/ffi.py wraps both sets.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -185,7 +185,7 @@ float compute_mse_loss(const std::vector<int64_t> &hist, const int start, const 
     return ppq_b200_compute_mse_loss(hist.data(), (int64_t)hist.size(), start, step, end);
 }
 
-// ---------------------------------------------------------------- B200-native extras (not in the reference table)
+// ---------------------------------------------------------------- H100-native extras (not in the reference table)
 void MinMax_Init(Tensor &mins, Tensor &maxs) {
     CheckTensor(mins, at::kFloat, "Min(Expect to be FP32)");
     CheckTensor(maxs, at::kFloat, "Max(Expect to be FP32)");
@@ -336,7 +336,7 @@ int get_variant(const std::string &kernel) { return ppq_b200_get_variant(kernel.
 #include "torch_binding_more.inc"
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-    m.doc() = "ppq_b200: B200-native drop-in for PPQ_Cuda_Impls";
+    m.doc() = "ppq_b200: H100-native drop-in for PPQ_Cuda_Impls";
     // the reference table, ppq/csrc/export.cc:9-33
     m.def("Histogram_T", Histogram_T, "Histogram_T");
     m.def("Histogram_Asymmetric_T", Histogram_Asymmetric_T, "Histogram_Asymmetric_T");
@@ -347,7 +347,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("QuantizeTensor_FC", QuantizeTensor_FC, "QuantizeTensor_FC");
     m.def("compute_mse_loss", compute_mse_loss, "compute_mse_loss");
     register_more(m);
-    // B200-native extras
+    // H100-native extras
     m.def("QuantizeTensor_toInt", QuantizeTensor_toInt, "QuantizeTensor_toInt");
     m.def("Multi_QuantizeTensor_LC", Multi_QuantizeTensor_LC, "Multi_QuantizeTensor_LC");
     m.def("Multi_QuantizeTensor_LT", Multi_QuantizeTensor_LT, "Multi_QuantizeTensor_LT");

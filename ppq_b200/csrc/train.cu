@@ -1,4 +1,4 @@
-// train.cu -- the training-pass helpers that share the scalar quantizer (sm_100a), behind the C ABI of include/ppq_b200.h.
+// train.cu -- the training-pass helpers that share the scalar quantizer (sm_90a), behind the C ABI of include/ppq_b200.h.
 // These are the "next" rows of the scope table (SURVEY.md §8f-2, §8f-4): callers on either side of the fake-quant path.
 //
 //   ppq_b200_linear_quant_t_backward / _c_backward   replace QuantizeTensor_LT_B / _LC_B (/root/reference/ppq/csrc/cuda/linear.cu:235-433)

@@ -1,6 +1,6 @@
 // variants.h -- run-time kernel variant selection (profiling / A-B benchmarking knob, see ppq_b200_set_variant).
 //   "linear_quant_t": 0 default (LDG.128, warp-contiguous segments, unroll by size) | 1 TMA-staged smem ring | 2 force 8 loads in flight
-//                     | 3 force 4 loads in flight on a persistent 148 x 8 grid
+//                     | 3 force 4 loads in flight on a persistent SM count x 8 grid
 //   "histogram":      0 default (two 1024-thr CTAs per SM, 2 loads in flight, unconditional red.shared + trash slot) | 1 generic-pointer atomicAdd
 //                     | 2 __match_any_sync aggregation | 3 global atomics like the reference | 4 the first layout (256-thr CTAs x 8 per SM)
 //                     | 5 the round-1 default (one 1024-thr CTA per SM, 4 loads in flight) | 6 two CTAs per SM, 4 loads in flight | 7, 8 clusters of 2 / 4 CTAs, DSMEM pre-reduction of the bins

@@ -25,7 +25,7 @@ non-quantable operation), except: a view of a known tensor shares its producer's
 passive operations upstream), and a Relu / Clip fed by an invisible operation fuses with it (refine.py:293-306).  Use the
 `Add` / `Concat` modules of this file when element-wise ops must be quantised and aligned like the reference's graph.
 
-B200-native addition: `collect=True` makes the executor hand the observed fp32 tensors of a whole forward to an ArenaCalibrator
+H100-native addition: `collect=True` makes the executor hand the observed fp32 tensors of a whole forward to an ArenaCalibrator
 (one multi-tensor launch per phase) instead of firing one observer launch per tensor.
 """
 from typing import Dict, List, Optional
@@ -536,8 +536,8 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     deferred='auto' (default) finds out during the first forward which observed tensors the network later overwrites in place
     (torchvision adds residuals with `out += identity`), observes those immediately and everything else in one multi-tensor launch;
     graphs=True captures one forward per phase -- network kernels, per-forward weight fake-quant and the collectors -- into a CUDA
-    graph and replays it for every batch (fixed batch shape).  Measured on B200 (ResNet-50, 8 x 32 images): capture + instantiate
-    costs more than it saves at 8-16 batches per phase (1330 vs 3124 imgs/s end to end), so it is off by default; it pays off for long
+    graph and replays it for every batch (fixed batch shape).  Capture + instantiate
+    costs more than it saves at 8-16 batches per phase, so it is off by default; it pays off for long
     calibration sets or when the same graph is reused across calls.
     to_device: a callable applied to every batch, or 'ring' for host tensors staged through the device's persistent DeviceBatchRing.
     trace: a list that receives (phase, batch index, host time, CUDA event, thread CPU time) before every batch and at the end of a phase --
@@ -631,7 +631,7 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
     (python -> binding -> allocator -> launch, 4.5-5 us x every config x every forward) disappears from the loop.
     fetchs=None measures on whole tensors, every quantable operation.  fetchs=4096 follows the reference to the letter: computing operations
     only (graphwise.py:112-113), `fetchs` elements per sample picked by the reference's seeded linear congruential indexer
-    (utils/fetch.py:4-23, seed 10086) -- pinned against the real function on the B200 (tests/test_gpu_graph_parity.py)."""
+    (utils/fetch.py:4-23, seed 10086) -- pinned against the real function on the GPU (tests/test_gpu_graph_parity.py)."""
     names = [n for n, op in executor.quantable_operations() if fetchs is None or op.kind in COMPUTING_OP]
     acc = {n: None for n in names}
     count = 0

@@ -29,7 +29,7 @@ class ComplieHelper:
         if not os.path.exists(_EXT_PATH):
             raise ImportError(
                 f'ppq_b200 native extension not found at {_EXT_PATH}. Build it in-tree first: `python -m ppq_b200.build` '
-                '(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.')
+                '(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.')
         spec = importlib.util.spec_from_file_location('ppq_b200._C', _EXT_PATH)
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
@@ -172,7 +172,7 @@ class CUDA:
     def Sync():
         torch.cuda.synchronize()
 
-    # ---- B200-native additions (no counterpart in the reference table) -------------------------------------------
+    # ---- H100-native additions (no counterpart in the reference table) -------------------------------------------
     @staticmethod
     def LinearQuantize_toInt(tensor, scales, offsets, channel_axis=None, minimum: int = -128, maximum: int = 127,
                              rounding: int = 0, out_bits: int = 8) -> torch.Tensor:

@@ -1,7 +1,7 @@
 """Install ppq_b200 into an unmodified OpenPPL/ppq checkout (drop-in boundary, SURVEY.md §8b).
 
     import ppq, ppq_b200.install
-    ppq_b200.install.install()            # CUDA_COMPLIER now serves the sm_100a extension; complie() is a no-op
+    ppq_b200.install.install()            # CUDA_COMPLIER now serves the sm_90a extension; complie() is a no-op
     with ppq.api.ENABLE_CUDA_KERNEL(): ...
 
 Everything ppq.core.ffi.CUDA calls (`CUDA_COMPLIER.CUDA_EXTENSION.<name>(...)`, /root/reference/ppq/core/ffi.py:78-344)
@@ -22,7 +22,7 @@ _TYPE_CHECK_SITES = (('ppq.quantization.optim.calibration', 'TorchHistObserver')
 
 
 def install(replace_observers: bool = True):
-    """Route ppq.core.ffi.CUDA to the sm_100a extension; with replace_observers also swap the 'minmax' / 'kl' / 'mse' / 'percentile'
+    """Route ppq.core.ffi.CUDA to the sm_90a extension; with replace_observers also swap the 'minmax' / 'kl' / 'mse' / 'percentile'
     observers for the device-resident ones (they need CUDA tensors: a CPU-path calibration of the real PPQ should call uninstall()
     first or pass False)."""
     import importlib

@@ -1,7 +1,7 @@
 """Calibration observers: the mirror of ppq/quantization/observer (/root/reference/ppq/quantization/observer/
-__init__.py:15-124, range.py:22-520, floating.py:11-144) on top of the sm_100a collectors.
+__init__.py:15-124, range.py:22-520, floating.py:11-144) on top of the sm_90a collectors.
 
-What changed versus the reference (results are the same, the data flow is B200-first):
+What changed versus the reference (results are the same, the data flow is H100-first):
   * observe() never appends to Python lists: every observer owns a slice of a device-resident *statistics arena*
     ({min, max} floats, int32 histogram bins) that the kernels accumulate into with atomics;
   * min and max are one fused pass (MinMax_T / MinMax_C), not value.min() + value.max();
@@ -203,7 +203,7 @@ class TorchHistObserver(TorchMinMaxObserver):
 
 class TorchMSEObserver(TorchHistObserver):
     """range.py:406-520: histogram-accelerated MSE search.  The grid search drives compute_mse_loss exactly like the
-    reference does with USING_CUDA_KERNEL=True (ffi.py:263-270 -> hist_mse.cc); histogram collection is the sm_100a kernel."""
+    reference does with USING_CUDA_KERNEL=True (ffi.py:263-270 -> hist_mse.cc); histogram collection is the sm_90a kernel."""
 
     def __init__(self, watch_on, quant_cfg: TensorQuantizationConfig, bins: int = OBSERVER_MSE_HIST_BINS, slot: StatSlot = None):
         super().__init__(watch_on, quant_cfg, hist_bins=bins, slot=slot)

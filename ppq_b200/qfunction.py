@@ -2,7 +2,7 @@
 __init__.py:10-61, linear.py:8-238, floating.py:7-120), CUDA branch only.
 
 Same names, same state / policy checks, same straight-through backward; the forward of every autograd Function calls the
-sm_100a kernels through ppq_b200.ffi.CUDA.  There is deliberately no torch fallback: CPU tensors raise.
+sm_90a kernels through ppq_b200.ffi.CUDA.  There is deliberately no torch fallback: CPU tensors raise.
 """
 import torch
 from torch.autograd import Function

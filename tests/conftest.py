@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100: pytest -m gpu)')
 
 
 def load_golden(name):

@@ -43,7 +43,7 @@ def load():
 
 
 def reference_cuda_extension():
-    """The reference's own CUDA extension compiled unmodified for sm_100a (oracle/build_ref.py), or None."""
+    """The reference's own CUDA extension compiled unmodified for sm_90a (oracle/build_ref.py), or None."""
     if not os.path.exists(REF_SO):
         return None
     spec = importlib.util.spec_from_file_location('PPQ_Cuda_Impls_ref', REF_SO)

@@ -1,4 +1,4 @@
-"""CPU twins of the three arithmetic shortcuts the sm_100a kernels take (ppq_b200/csrc/common.cuh, ops.cuh), checked here without a GPU:
+"""CPU twins of the three arithmetic shortcuts the sm_90a kernels take (ppq_b200/csrc/common.cuh, ops.cuh), checked here without a GPU:
 
   1. ExactDiv: x / s through a hoisted reciprocal and two Markstein corrections == the IEEE fp32 quotient (exact rational arithmetic);
   2. the "+ .5" rounding modes evaluated in fp32 (floor / ceil + fraction test) == the reference's double formulation (the oracle);

@@ -4,7 +4,7 @@ pipeline (TRT_INT8 quantizer's own pass list on a programmatically built BaseGra
     four observers, aligned Add inputs, baked weights and the quantised network output -- so the CPU arm is a pinned port;
   * ppq_b200.executor's topology passes (fusion + simplify, which need no GPU) give the same states / dominators / observed set;
   * where the reference checkout is present, the fixture is regenerated live and must not have drifted.
-The GPU twin (tests/test_gpu_graph_parity.py) runs the real reference package on the B200 through ppq_b200.install.install().
+The GPU twin (tests/test_gpu_graph_parity.py) runs the real reference package on the GPU through ppq_b200.install.install().
 """
 import json
 

@@ -1,4 +1,4 @@
-"""Multi-GPU / multi-device tests (need >= 2 visible GPUs: `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`; skipped on a 1-GPU box).
+"""Multi-GPU / multi-device tests (need >= 2 visible GPUs: `python -m pytest tests/test_gpu_multi.py -m gpu`; skipped on a 1-GPU machine).
 
   * BASELINE config 5's flow over REAL NCCL: two ranks, one per GPU, each calibrating its sample shard of a YOLOv5s-like activation set
     through ArenaCalibrator (multi-tensor launches, the two all-reduces of SURVEY 8e) -- all four observer algorithms -- must reproduce the
@@ -58,7 +58,7 @@ def _worker(rank, world, port, out_dir):
 
 
 def test_config5_two_ranks_over_nccl_equal_the_single_process_calibration(tmp_path):
-    if torch.cuda.device_count() < 2: pytest.skip('needs 2 GPUs (gpurun --gpus 2)')
+    if torch.cuda.device_count() < 2: pytest.skip('needs 2 GPUs')
     import torch.multiprocessing as mp
     from ppq_b200.calibration import ArenaCalibrator
     world, port = 2, _free_port()
@@ -76,7 +76,7 @@ def test_config5_two_ranks_over_nccl_equal_the_single_process_calibration(tmp_pa
 
 
 def test_one_process_two_devices():
-    if torch.cuda.device_count() < 2: pytest.skip('needs 2 GPUs (gpurun --gpus 2)')
+    if torch.cuda.device_count() < 2: pytest.skip('needs 2 GPUs')
     from ppq_b200.ffi import extension
     ext = extension()
     res = []

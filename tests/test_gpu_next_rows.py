@@ -1,19 +1,16 @@
 """GPU parity of the "next" rows (SURVEY.md §8f): Quantile_T / Isotone_T by radix select, LSQ backward, float backward,
-TensorClip, RoundingLoss -- against the reference's own CUDA kernels (oracle/_ref) where present, and against the oracle /
-the torch formulas of the reference's test (tests/test_cuda_kernel.py:66-143) otherwise.
+TensorClip, RoundingLoss -- against the reference's own CUDA kernels (their recorded results, tests/refcuda.py), against the oracle
+and against the torch formulas of the reference's test (tests/test_cuda_kernel.py:66-143).
 Element-wise outputs must be bit-identical; scalar fp32 reductions (grad_s, loss) to 1e-4 relative (the reference's own bar is SNR 1e-3)."""
-import importlib.util
-import os
 from math import sqrt
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+import refcuda
 
 pytestmark = pytest.mark.gpu
-REF_SO = os.path.join(ROOT, 'oracle', '_ref', 'PPQ_Cuda_Impls_ref.so')
 
 
 @pytest.fixture(scope='module')
@@ -24,16 +21,11 @@ def ext():
     return extension()
 
 
-@pytest.fixture(scope='module')
-def ref():
+@pytest.fixture
+def ref(request):
     if not torch.cuda.is_available():
         pytest.skip('no CUDA device')
-    if not os.path.exists(REF_SO):
-        return None
-    spec = importlib.util.spec_from_file_location('PPQ_Cuda_Impls_ref', REF_SO)
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
+    return refcuda.reference(request.node.nodeid)
 
 
 def same_bits(a, b):

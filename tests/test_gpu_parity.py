@@ -1,8 +1,8 @@
-"""GPU parity: the sm_100a kernels (through the torch binding AND through the raw C ABI) against the CPU oracle and the
+"""GPU parity: the sm_90a kernels (through the torch binding AND through the raw C ABI) against the CPU oracle and the
 golden vectors of the real reference.  Bit-exact for every integer / fake-quant output (the reference's own bar:
 tests/test_cuda_kernel.py:35-37 `diff.abs().max() != 0 -> fail`).
 
-Run on the B200 box:  python -m pytest tests -m gpu -x -q
+Run on an H100:  python -m pytest tests -m gpu -x -q
 """
 import ctypes
 import hashlib

@@ -176,20 +176,15 @@ def test_compute_mse_loss_vs_reference_cpp(oracle):
 
 
 def test_compute_mse_loss_vs_live_reference_build(oracle):
-    """When oracle/_ref/hist_mse_ref.so (the reference's hist_mse.cc compiled in place) is present, fuzz against it."""
-    import ctypes
-    so = os.path.join(os.path.dirname(GOLDEN), '..', 'oracle', '_ref', 'hist_mse_ref.so')
-    if not os.path.exists(so):
-        pytest.skip('oracle/_ref not built on this machine')
-    lib = ctypes.CDLL(so)
-    lib.ref_compute_mse_loss.restype = ctypes.c_float
-    lib.ref_compute_mse_loss.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+    """Fuzz against the reference's hist_mse.cc (compiled in place by oracle/build_ref.py): tests/golden/mse_loss_fuzz.npz holds what it
+    returned for these 200 seeded histograms (ref_compute_mse_loss of oracle/ref_shim_hist_mse.cc, same loop)."""
+    want = load_golden('mse_loss_fuzz.npz')['vals']
     r = np.random.RandomState(99)
-    for _ in range(200):
+    for i in range(200):
         nb = int(r.choice([16, 100, 2048]))
         h = r.randint(0, 5000, size=nb).astype(np.int64)
         step = int(r.randint(1, 9)); start = int(r.randint(0, nb // 2)); end = start + int(r.randint(1, 300)) * step
-        assert np.float32(oracle.compute_mse_loss(h, start, step, end)) == np.float32(lib.ref_compute_mse_loss(h.ctypes.data, nb, start, step, end))
+        assert np.float32(oracle.compute_mse_loss(h, start, step, end)) == want[i], (nb, start, step, end)
 
 
 def test_fp8_restatement_sanity(oracle):
@@ -220,8 +215,8 @@ def test_quantile_indices(oracle):
 
 
 def test_fp8_and_histogram_vs_reference_cuda_kernels(oracle):
-    """Vectors produced ON THE B200 BY THE REFERENCE'S OWN CUDA KERNELS (oracle/_ref/PPQ_Cuda_Impls_ref.so; written by
-    tests/test_gpu_vs_reference_cuda.py, committed under tests/golden/ref_cuda_*.npz): this pins the C restatement of the paths that have
+    """Vectors produced ON THE GPU BY THE REFERENCE'S OWN CUDA KERNELS (upstream ppq/csrc built by oracle/build_ref.py; committed under
+    tests/golden/ref_cuda_*.npz): this pins the C restatement of the paths that have
     no CPU implementation upstream -- QuantizeTensor_FT (all tie / subnormal / saturation / special-value cases, two rounding modes,
     four formats) and Histogram_T."""
     import re

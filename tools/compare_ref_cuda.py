@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Ours vs the reference's own CUDA kernels (oracle/_ref/PPQ_Cuda_Impls_ref.so: ppq/csrc compiled unmodified for sm_100a) on the same B200,
+"""Ours vs the reference's own CUDA kernels (oracle/_ref/PPQ_Cuda_Impls_ref.so: ppq/csrc compiled unmodified for sm_90a) on the same GPU,
 same tensors, CUDA events, rotating buffers > L2.  A measurement tool (not part of bench.py): output is kept in profiles/."""
 import importlib.util
 import json
@@ -67,7 +67,7 @@ def main():
     out = os.path.join(ROOT, 'gpurun_out', 'vs_reference_kernels.md')
     os.makedirs(os.path.dirname(out), exist_ok=True)
     with open(out, 'w') as f:
-        f.write(f'# ours vs the reference\'s own CUDA kernels (compiled for sm_100a) on the same B200 -- {torch.cuda.get_device_name(0)}\n\n')
+        f.write(f'# ours vs the reference\'s own CUDA kernels (compiled for sm_90a) on the same GPU -- {torch.cuda.get_device_name(0)}\n\n')
         f.write(f'50.3 M fp32 elements per call, {nbuf} rotating buffers (1.2 GB), CUDA events; peak = {PEAK:.0f} GB/s (measured copy).\n\n')
         f.write('| op | ours us | ours GB/s | ours % peak | reference us | reference GB/s | reference % peak | speed-up |\n|---|---|---|---|---|---|---|---|\n')
         for r in rows: f.write(f'| {r[0]} | {r[1]:.1f} | {r[2]:.0f} | {r[3]:.1%} | {r[4]:.1f} | {r[5]:.0f} | {r[6]:.1%} | {r[7]:.1f}x |\n')

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Runs on the B200 box under gpurun: GPU parity tests, smoke, a short bench and the ncu launch list.  Outputs -> gpurun_out/.
+# GPU parity tests, smoke, a short bench and the ncu launch list, run on one GPU machine; outputs go to the output directory below.
 mkdir -p gpurun_out
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,power.draw,memory.total --format=csv > gpurun_out/gpu.txt 2>&1
 python -m pytest tests -m gpu -x -q > gpurun_out/tests.log 2>&1; echo "pytest exit $?" >> gpurun_out/tests.log

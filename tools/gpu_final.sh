@@ -1,5 +1,5 @@
 #!/bin/bash
-# Round-end verification on the B200 box: parity tests, smoke, kernel micro-benchmarks, both bench arms, ncu launch list of the timed
+# Round-end verification on the GPU: parity tests, smoke, kernel micro-benchmarks, both bench arms, ncu launch list of the timed
 # region and one full capture of the (rewritten) multi-tensor weight fake-quant kernel.  Everything lands in gpurun_out/.
 mkdir -p gpurun_out
 timeout 500 python -m pytest tests -m gpu -q 2>&1 | grep -v "^  \|^$" | cut -c1-300 | tail -8

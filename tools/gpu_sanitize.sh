@@ -1,5 +1,5 @@
 #!/bin/bash
-# Runs on the B200 box under gpurun: compute-sanitizer memcheck over the GPU parity tests of OUR kernels (the comparison against the
+# compute-sanitizer memcheck over the GPU parity tests of OUR kernels (the comparison against the
 # reference's own CUDA build is excluded: its kernels are not ours to fix), then racecheck over the shared-memory kernels.
 # PYTORCH_NO_CUDA_MEMORY_CACHING=1: every tensor is its own cudaMalloc, so an out-of-bounds access cannot hide inside torch's pool.
 mkdir -p gpurun_out

@@ -32,7 +32,7 @@ def short(name):
 def main():
     objs = sorted(glob.glob(os.path.join(ROOT, 'ppq_b200', '_build', '*.o')))
     wanted = sys.argv[1:]                                               # optional substrings to filter kernel names
-    print('# SASS opcode histogram per kernel (sm_100a, cuobjdump -sass of ppq_b200/_build/*.o)\n')
+    print('# SASS opcode histogram per kernel (sm_90a, cuobjdump -sass of ppq_b200/_build/*.o)\n')
     print('Columns: total instructions, then the opcodes that characterise the kernel. `LDG.128` counts every 128-bit global load '
           '(`LDG.E.128*`, incl. the `.NA` no-allocate / `.CONSTANT` forms), `ATOMS` the shared-memory atomics (`ATOMS.POPC.INC` = hardware-aggregated '
           'increment), `RED/ATOMG` global reductions, `RCP/FCHK` the reciprocal and the IEEE-division range check (FCHK only appears in the '
