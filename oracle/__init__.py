@@ -235,14 +235,19 @@ def numerical_round(value: float, mode: int = RND_HALF_EVEN) -> int:
     raise ValueError('Unexpected rounding policy found.')
 
 
-def round_to_power_of_2(value: float, mode: int = RND_UP) -> float:
+def round_to_power_of_2(value: float, mode: int = RND_UP, ieee: bool = False) -> float:
+    """ieee=True: NaN and +-inf, where the reference raises (math.ceil / Decimal of log2(nan) or log2(inf)), are returned unchanged -- what the
+    device computes for them (DESIGN.md §2)."""
     if value == 0: return 0
+    if ieee and not math.isfinite(value): return value
     sign = 1 if value >= 0 else -1
     return sign * float(pow(2, numerical_round(math.log2(sign * value), mode)))
 
 
 # ---- minmax_to_scale_offset: ppq/quantization/observer/range.py:22-75 (Python doubles) -------------
-def minmax_to_scale_offset(min_val, max_val, qmin, qmax, symmetrical, power_of_2=False, scale_threshold=1e-8):
+def minmax_to_scale_offset(min_val, max_val, qmin, qmax, symmetrical, power_of_2=False, scale_threshold=1e-8, ieee=False):
+    """ieee=True: where the reference raises -- int(nan) for the offset of a non-finite asymmetric range, the power-of-two of a NaN or inf
+    scale -- return the IEEE result instead (offset NaN, scale unchanged), which is what the device computes."""
     min_val, max_val = float(min_val), float(max_val)
     if min_val > 0: min_val = 0.0
     if max_val < 0: max_val = 0.0
@@ -253,9 +258,10 @@ def minmax_to_scale_offset(min_val, max_val, qmin, qmax, symmetrical, power_of_2
     else:
         scale = float(max_val - min_val) / (qmax - qmin)
         scale = max(scale, scale_threshold)
-        offset = numerical_round(-min_val / scale)
+        q = -min_val / scale
+        offset = q if (ieee and not math.isfinite(q)) else numerical_round(q)
     if power_of_2:
-        scale = round_to_power_of_2(scale, RND_UP)
+        scale = round_to_power_of_2(scale, RND_UP, ieee)
     return scale, offset
 
 
@@ -266,11 +272,11 @@ def kl_divergence(p, q, eps=1e-30):
     return torch.dot(p, torch.log10(p + eps) - torch.log10(q + eps)).item()
 
 
-def kl_search(hist, hist_scale, num_of_bits=8, power_of_2=False, scale_threshold=1e-8, return_losses=False):
+def kl_search(hist, hist_scale, num_of_bits=8, power_of_2=False, scale_threshold=1e-8, return_losses=False, ieee=False):
     """Candidate clip points bin_range = quant_bins, 2*quant_bins, ... (< bins + quant_bins - 1).  For each:
     P = first bin_range bins with the tail folded into the last one, / total;  Q = the same bins merged into
     quant_bins groups, each group's mass spread evenly over its non-empty bins, normalised;  loss = KL(P||Q) in
-    fp64 log10.  First minimum wins.  fp32 tensors / torch CPU reductions exactly as upstream."""
+    fp64 log10.  First minimum wins.  fp32 tensors / torch CPU reductions exactly as upstream.  ieee: see minmax_to_scale_offset."""
     import torch
     h = torch.as_tensor(np.asarray(hist)).float().clone()
     bins = h.numel()
@@ -296,19 +302,28 @@ def kl_search(hist, hist_scale, num_of_bits=8, power_of_2=False, scale_threshold
         losses.append(loss)
         if best is None or loss < best_loss:
             best, best_loss = bin_range, loss
-    scale = (best / bins) * hist_scale * (bins / quant_bins)
-    scale = max(scale, scale_threshold)
-    if power_of_2:
-        scale = round_to_power_of_2(scale, RND_HALF_UP)
+    scale = kl_scale(best, bins, hist_scale, num_of_bits, power_of_2, scale_threshold, ieee)
     if return_losses:
         return scale, 0, best, losses
     return scale, 0
 
 
+def kl_scale(best, bins, hist_scale, num_of_bits=8, power_of_2=False, scale_threshold=1e-8, ieee=False):
+    """The scale of the winning bin range (range.py:271-282): clamp to the minimum scale, power-of-two with the exponent rounded half-up."""
+    quant_bins = 2 ** (num_of_bits - 1)
+    scale = (best / bins) * hist_scale * (bins / quant_bins)
+    scale = max(scale, scale_threshold)
+    if power_of_2:
+        scale = round_to_power_of_2(scale, RND_HALF_UP, ieee)
+    return scale
+
+
 # ---- MSE search: TorchMSEObserver.hist_to_scale_offset, range.py:456-520 ---------------------------
-def mse_search(hist, hist_scale, vmin, qmin, qmax, symmetrical, power_of_2=False, interval=8, loss_fn=None):
+def mse_search(hist, hist_scale, vmin, qmin, qmax, symmetrical, power_of_2=False, interval=8, loss_fn=None, scale_threshold=1e-8,
+               ieee=False):
     """loss_fn defaults to the C++ compute_mse_loss restatement (fp32 accumulate; what CUDA.compute_mse_loss is).
-    Pass `mse_loss_python_twin` to follow the USING_CUDA_KERNEL=False branch (Python doubles, range.py:431-454)."""
+    Pass `mse_loss_python_twin` to follow the USING_CUDA_KERNEL=False branch (Python doubles, range.py:431-454).
+    scale_threshold: OBSERVER_MIN_SCALE_MANUL_OVERRIDE, handed to minmax_to_scale_offset; ieee: see there."""
     loss_fn = loss_fn or compute_mse_loss
     hist = [int(v) for v in np.asarray(hist).tolist()]
     bins = len(hist)
@@ -334,7 +349,7 @@ def mse_search(hist, hist_scale, vmin, qmin, qmax, symmetrical, power_of_2=False
         lo, hi = -(e0 * hist_scale), (e0 * hist_scale)
     else:
         lo, hi = (s0 * hist_scale) + vmin, (e0 * hist_scale) + vmin
-    return minmax_to_scale_offset(lo, hi, qmin, qmax, symmetrical, power_of_2)
+    return minmax_to_scale_offset(lo, hi, qmin, qmax, symmetrical, power_of_2, scale_threshold, ieee)
 
 
 def mse_loss_python_twin(hist, start, step, end):

@@ -135,24 +135,39 @@ def shared_stager(device, columns: int) -> DescriptorStager:
     return _STAGERS[key]
 
 
+ARENA_MAX_HIST_BINS = 12287          # the multi-tensor histogram keeps (bins + 1) private counters in 48 KB of shared memory
+
+
 class ArenaCalibrator:
     """method:  'minmax'      one phase: fused min/max                       -> MinMax_To_Scale_Offset
-                'kl'          + phase 2: 4096-bin histogram                  -> KL_Search
+                'kl'          + phase 2: 4096-bin histogram                  -> KL_Search (symmetric configs only, as upstream)
                 'mse'         + phase 2: 2048-bin histogram                  -> MSE_Search (symmetric configs; range.py:406-520)
                 'percentile'  one phase: Quantile_T of every tensor and batch (ONE multi-tensor select per forward), fp32 mean over the
-                              batches in sample order                        -> MinMax_To_Scale_Offset   (range.py:312-403)"""
+                              batches in sample order                        -> MinMax_To_Scale_Offset   (range.py:312-403)
+    All T tensors share one per-tensor config: range (quant_min, quant_max, num_of_bits), symmetrical, power_of_2 and min_scale.  The
+    histogram of both two-phase methods is symmetric (|x| binned from 0), so asymmetric 'kl' / 'mse' are refused, as are more than
+    ARENA_MAX_HIST_BINS bins."""
 
     def __init__(self, num_tensors: int, device, bins: int = None, num_of_bits: int = 8,
                  quant_min: int = -128, quant_max: int = 127, power_of_2: bool = False, min_scale: float = OBSERVER_MIN_SCALE,
-                 method: str = 'kl', group=None, percentile: float = OBSERVER_PERCENTILE, select_cap: int = 1 << 16):
+                 method: str = 'kl', group=None, percentile: float = OBSERVER_PERCENTILE, select_cap: int = 1 << 16,
+                 symmetrical: bool = True):
         from .ffi import extension
         if method not in ('kl', 'minmax', 'mse', 'percentile'):
             raise ValueError(f"ArenaCalibrator: unknown observer algorithm {method!r} (expected 'kl', 'minmax', 'mse' or 'percentile')")
+        if method == 'kl' and not symmetrical:
+            raise PermissionError('KL observer is not designed for ASYMMETRICAL quantization')
+        if method == 'mse' and not symmetrical:
+            raise ValueError('ArenaCalibrator: the arena histogram is symmetric; asymmetric mse calibration needs the per-observer '
+                             'RuntimeCalibrationPass')
         if bins is None: bins = OBSERVER_MSE_HIST_BINS if method == 'mse' else OBSERVER_KL_HIST_BINS
+        if method in ('kl', 'mse') and bins > ARENA_MAX_HIST_BINS:
+            raise ValueError(f'ArenaCalibrator: {bins} histogram bins, the multi-tensor histogram holds at most {ARENA_MAX_HIST_BINS}; '
+                             'use RuntimeCalibrationPass for larger histograms')
         self.ext = extension()
         self.T, self.bins, self.device, self.group = num_tensors, bins, torch.device(device), group
         self.num_of_bits, self.quant_min, self.quant_max = num_of_bits, quant_min, quant_max
-        self.power_of_2, self.min_scale, self.method = power_of_2, min_scale, method
+        self.power_of_2, self.min_scale, self.method, self.symmetrical = power_of_2, min_scale, method, symmetrical
         self.percentile, self.select_cap = percentile, select_cap
         self.minmax = torch.empty(num_tensors, 2, dtype=torch.float32, device=self.device)
         two_phase = method in ('kl', 'mse')
@@ -247,7 +262,7 @@ class ArenaCalibrator:
     @torch.no_grad()
     def end_phase(self):
         """Exchange + render of the finished phase.  Returns True when calibration is complete."""
-        sym = True                                                       # the arena serves per-tensor symmetric activation configs
+        sym = self.symmetrical
         if self.method == 'percentile':
             if not self._pct: raise ValueError('Can not render quantization config yet, Observer data collator is empty.')
             rows = torch.stack(self._pct, dim=1)                         # [T, batches, 2]

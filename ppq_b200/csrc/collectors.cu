@@ -307,16 +307,16 @@ histogram_cluster_kernel(const float *__restrict__ x, int64_t n, BinParams bp, i
     cluster.sync();                                                     // nobody exits while a peer still reads its shared memory
 }
 
-// hist_scale read from device memory (phase 2 without a host round trip)
-template <int VARIANT>
-__global__ void __launch_bounds__(kHistThreads, 2)
+// hist_scale read from device memory (phase 2 without a host round trip); VARIANT 3 (global atomics) above kMaxSmemBins bins
+template <int VARIANT, int TPB = kHistThreads, int MINB = 2>
+__global__ void __launch_bounds__(TPB, MINB)
 histogram_dscale_kernel(const float *__restrict__ x, int64_t n, const float *__restrict__ hist_scale, int clip, int bins,
                         int32_t *__restrict__ hist) {
     extern __shared__ int sh[];
     hist_zero<VARIANT>(sh, bins);
     Counter<VARIANT> cnt(sh, hist, bins);
     const SymBin bin(__ldg(hist_scale), bins, clip != 0);
-    hist_stream<VARIANT, SymBin, 2>(x, n, (int64_t)blockIdx.x * kHistThreads + threadIdx.x, (int64_t)gridDim.x * kHistThreads, bin, cnt);
+    hist_stream<VARIANT, SymBin, 2>(x, n, (int64_t)blockIdx.x * TPB + threadIdx.x, (int64_t)gridDim.x * TPB, bin, cnt);
     hist_flush<VARIANT>(sh, bins, hist);
 }
 
@@ -462,7 +462,12 @@ int ppq_b200_histogram_asym_t(const float *x, int64_t n, float vmin, float vmax,
 
 int ppq_b200_histogram_t_dscale(const float *x, int64_t n, const float *hist_scale_dev, int clip_outliers, int32_t *hist,
                                 int64_t bins, void *stream) {
-    if (n <= 0 || !x || !hist || !hist_scale_dev || bins <= 0 || bins > kMaxSmemBins) return (int)cudaErrorInvalidValue;
+    if (n <= 0 || !x || !hist || !hist_scale_dev || bins <= 0 || bins > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+    if (bins > kMaxSmemBins) {                     // the private bins do not fit: count with global atomics, as launch_hist does for Histogram_T
+        histogram_dscale_kernel<3, kThreads, 1><<<grid_for(n, kThreads, 16, 8), kThreads, 0, (cudaStream_t)stream>>>(
+            x, n, hist_scale_dev, clip_outliers, (int)bins, hist);
+        return (int)cudaGetLastError();
+    }
     const int grid = hist_grid(n, (int)bins) * 2 > sm_count() * 2 ? sm_count() * 2 : hist_grid(n, (int)bins) * 2;
     histogram_dscale_kernel<0><<<grid, kHistThreads, (size_t)(bins + 1) * sizeof(int), (cudaStream_t)stream>>>(
         x, n, hist_scale_dev, clip_outliers, (int)bins, hist);

@@ -20,25 +20,51 @@ namespace ppqb {
 // ppq_numerical_round(v, ROUND_HALF_EVEN) on a double (utils/round.py:78: Decimal.quantize half-even == rint).
 __device__ __forceinline__ double round_half_even(double v) { return rint(v); }
 
+// log2(v) as a correctly rounded log2 returns it, for v whose log2 lies next to the anchor `a` (an integer or a half-integer): CUDA's log2 may be
+// one ulp off, which moves ceil() when the rounded value should be exactly an integer and half-up when it should be exactly k + 0.5.
+// log2(v) = a + log2(v^2 / 2^(2a)) / 2 with v^2 exact as a double-double (fma) and 2a an integer, so the tiny correction is accurate to a few
+// ulps of itself and the only rounding that matters is the final a + delta.
+__device__ __forceinline__ double log2_near(double v, double a) {
+    const int two_a = (int)(2.0 * a);
+    const double p = v * v, pe = fma(v, v, -p);
+    const double q = ldexp(p, -two_a), qe = ldexp(pe, -two_a);        // q in [0.5, 2]: q - 1 is exact
+    return a + 0.5 * log1p((q - 1.0) + qe) / 0.69314718055994530942;
+}
+
 // ppq_round_to_power_of_2 (utils/round.py:115-135): 2^round(log2(x)); ROUND_UP = ceil, ROUND_HALF_UP on the exponent.
 // Exact powers of two are recognised from the binary exponent (math.log2 is exact on them); everything else follows the Python formula
 // on the double log2, so a value a few ulps above a power of two rounds the way math.log2 + ceil() does.  The result is built with ldexp.
 // Ties of the HALF_UP policy: Decimal ROUND_HALF_UP for value > 0 (2.5 -> 3) and ROUND_HALF_DOWN for value <= 0 (-9.5 -> -9,
 // utils/round.py:80-82) -- both send an exact .5 to floor + 1.
+// NaN and +-inf, where math.log2 + ceil() / Decimal raise upstream, come back unchanged: the IEEE result, never a finite power of two.
 __device__ __forceinline__ double pow2_round(double v, bool half_up) {
     if (v == 0.0) return 0.0;
+    if (!isfinite(v)) return v;
     const double sign = v >= 0.0 ? 1.0 : -1.0;
+    const double av = sign * v;
     int e2;
-    const double m = frexp(sign * v, &e2);                             // |v| = m * 2^e2, m in [0.5, 1)
+    const double m = frexp(av, &e2);                                    // |v| = m * 2^e2, m in [0.5, 1)
+    const bool refine = av > 1e-150 && av < 1e150;                      // v^2 stays a normal double
     int e;
     if (m == 0.5) e = e2 - 1;                                           // exact power of two
     else {
-        const double l = log2(sign * v);
-        if (!half_up) e = (int)ceil(l);
-        else { const double f = floor(l); e = (l - f >= 0.5) ? (int)f + 1 : (int)f; }
+        double l = log2(av);
+        if (!half_up) {
+            const double n = rint(l);
+            if (refine && fabs(l - n) < 1e-9) l = log2_near(av, n);     // only an integer boundary moves ceil()
+            e = (int)ceil(l);
+        } else {
+            const double h = floor(l) + 0.5;
+            if (refine && fabs(l - h) < 1e-9) l = log2_near(av, h);     // only a half-integer boundary moves half-up
+            const double f = floor(l); e = (l - f >= 0.5) ? (int)f + 1 : (int)f;
+        }
     }
     return sign * ldexp(1.0, e);
 }
+
+// Python's max(a, b) (`b if b > a else a`): unlike fmax it keeps a NaN first argument, so a NaN range gives a NaN scale as in range.py.
+// The result depends on the argument order; every call keeps the order of the Python expression it replaces.
+__device__ __forceinline__ double py_max(double a, double b) { return (b > a) ? b : a; }
 
 struct ScaleOffset { double scale, offset; };
 __device__ __forceinline__ ScaleOffset minmax_to_scale_offset_dev(double mn, double mx, int qmin, int qmax, bool sym, bool pow2,
@@ -48,12 +74,12 @@ __device__ __forceinline__ ScaleOffset minmax_to_scale_offset_dev(double mn, dou
     ScaleOffset r;
     const double levels = (double)(qmax - qmin);
     if (sym) {
-        const double range = 2.0 * fmax(fabs(mx), fabs(mn));
-        r.scale = fmax(range / levels, min_scale);
+        const double range = 2.0 * py_max(fabs(mx), fabs(mn));
+        r.scale = py_max(range / levels, min_scale);
         r.offset = 0.0;
     } else {
         const double range = mx - mn;
-        r.scale = fmax(range / levels, min_scale);
+        r.scale = py_max(range / levels, min_scale);
         r.offset = round_half_even(-mn / r.scale);
     }
     if (pow2) r.scale = pow2_round(r.scale, false);
@@ -75,7 +101,7 @@ __global__ void hist_scale_kernel(const float *__restrict__ minmax, int64_t coun
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
     const double mn = (double)minmax[2 * i], mx = (double)minmax[2 * i + 1];
-    const double range = sym ? fmax(fabs(mx), fabs(mn)) : (mx - mn);
+    const double range = sym ? py_max(fabs(mx), fabs(mn)) : (mx - mn);
     hs[i] = (float)(range / (double)bins);
 }
 
@@ -195,10 +221,10 @@ kl_search_kernel(const int32_t *__restrict__ hist_arena, int bins, const float *
         double hs;
         if (minmax_arena) {
             const double mn = (double)minmax_arena[2 * blockIdx.x], mx = (double)minmax_arena[2 * blockIdx.x + 1];
-            hs = fmax(fabs(mx), fabs(mn)) / (double)bins;            // the Python double of range.py:294-300
+            hs = py_max(fabs(mx), fabs(mn)) / (double)bins;            // the Python double of range.py:294-300
         } else hs = (double)hist_scale_arena[blockIdx.x];
         double scale = ((double)s_best / (double)bins) * hs * ((double)bins / (double)quant_bins);
-        scale = fmax(scale, min_scale);
+        scale = py_max(scale, min_scale);
         if (pow2) scale = pow2_round(scale, true);
         scale_out[blockIdx.x] = (float)scale;
         if (best_out) best_out[blockIdx.x] = s_best;
@@ -308,10 +334,10 @@ kl_search_warp_kernel(const int32_t *__restrict__ hist_arena, int bins, const fl
         double hs;
         if (minmax_arena) {
             const double mn = (double)minmax_arena[2 * blockIdx.x], mx = (double)minmax_arena[2 * blockIdx.x + 1];
-            hs = fmax(fabs(mx), fabs(mn)) / (double)bins;
+            hs = py_max(fabs(mx), fabs(mn)) / (double)bins;
         } else hs = (double)hist_scale_arena[blockIdx.x];
         double scale = ((double)s_best / (double)bins) * hs * ((double)bins / (double)quant_bins);
-        scale = fmax(scale, min_scale);
+        scale = py_max(scale, min_scale);
         if (pow2) scale = pow2_round(scale, true);
         scale_out[blockIdx.x] = (float)scale;
         if (best_out) best_out[blockIdx.x] = s_best;
@@ -353,7 +379,7 @@ mse_search_kernel(const int32_t *__restrict__ hist_arena, int bins, const float 
     __syncthreads();
     const float ftotal = (float)s_total;
     const double vmin = (double)minmax_arena[2 * blockIdx.x], vmax = (double)minmax_arena[2 * blockIdx.x + 1];
-    const double hs = (sym ? fmax(fabs(vmax), fabs(vmin)) : (vmax - vmin)) / (double)bins;      // python doubles, range.py:294-300
+    const double hs = (sym ? py_max(fabs(vmax), fabs(vmin)) : (vmax - vmin)) / (double)bins;      // python doubles, range.py:294-300
     const int levels = (qmax - qmin) + 1;
     const int S = bins / levels;                                       // steps 1..S
     // candidate enumeration, in the reference's order: 0 = the min-max fallback (start 0, step S+1); then (start_i, step) row-major
@@ -383,6 +409,8 @@ mse_search_kernel(const int32_t *__restrict__ hist_arena, int bins, const float 
     if (threadIdx.x == 0) {
         float bl = best_loss[0]; int bi = best_idx[0];
         for (int w = 1; w < kMseThreads / 32; w++) if (best_loss[w] < bl || (best_loss[w] == bl && best_idx[w] < bi)) { bl = best_loss[w]; bi = best_idx[w]; }
+        // an empty histogram makes every loss 0/0 = NaN: nothing compares below the first candidate, so python's min() keeps it
+        if (bi == 0x7fffffff) bi = 0;
         int start, step;
         if (bi == 0) { start = 0; step = S + 1; } else { start = sym ? 0 : ((bi - 1) / S) * interval; step = (bi - 1) % S + 1; }
         const int end = start + levels * step;
@@ -421,8 +449,10 @@ int ppq_b200_kl_search(const int32_t *hist_arena, int64_t count, int64_t bins, c
         return (int)cudaErrorInvalidValue;
     if (num_of_bits < 2 || num_of_bits > 16) return (int)cudaErrorInvalidValue;
     const int64_t qb = 1ll << (num_of_bits - 1);
-    if (bins < qb || bins > 16384) return (int)cudaErrorInvalidValue;  // OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE: any multiple of the quant bins works
-    if (bins <= kKlMemoBins && bins % qb == 0 && variant_of(kVarKlSearch) == 0) {        // one warp per candidate
+    // OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE: any multiple of the quant bins up to 16384.  Other counts fail upstream: the candidate loop reaches a
+    // bin range beyond the histogram and p_hist[:bin_range].copy_(histogram[:bin_range]) raises (range.py:250).
+    if (bins < qb || bins > 16384 || bins % qb != 0) return (int)cudaErrorInvalidValue;
+    if (bins <= kKlMemoBins && variant_of(kVarKlSearch) == 0) {        // one warp per candidate
         const size_t ncand = (size_t)(bins / qb);
         const size_t plen = (size_t)(bins + 1 > kKlwThreads ? bins + 1 : kKlwThreads);
         const size_t smem_w = (((size_t)bins * 4 + 7) & ~(size_t)7) + plen * 8 + (size_t)bins * 8 + ((ncand + 1) & ~(size_t)1) * 8 +

@@ -526,6 +526,29 @@ def prefetch_to_device(batches, to_device, device):
         yield y
 
 
+def arena_settings(cfgs, method: str) -> dict:
+    """The ArenaCalibrator arguments that every observed config asks for, read the way the per-config observers read them
+    (ppq_b200.observer): range, bits, symmetry, power-of-two, OBSERVER_MIN_SCALE_MANUL_OVERRIDE, the KL bin override and the percentile
+    override.  One calibrator serves all tensors, so configs that differ in any of these -- or per-channel ones -- are refused."""
+    from .core import (OBSERVER_KL_HIST_BINS, OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE, OBSERVER_MSE_HIST_BINS, OBSERVER_PERCENTILE,
+                       OBSERVER_PERCENTILE_MANUL_OVERRIDE, QuantizationProperty as P)
+    found = {}
+    for c in cfgs:
+        if not c.policy.has_property(P.PER_TENSOR):
+            raise ValueError('calibrate_arena serves per-tensor activation configs only; use RuntimeCalibrationPass for per-channel ones')
+        if method == 'kl': bins = c.detail.get(OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE, OBSERVER_KL_HIST_BINS)
+        else: bins = OBSERVER_MSE_HIST_BINS if method == 'mse' else None
+        key = dict(quant_min=c.quant_min, quant_max=c.quant_max, num_of_bits=c.num_of_bits, symmetrical=c.policy.has_property(P.SYMMETRICAL),
+                   power_of_2=c.policy.has_property(P.POWER_OF_2), min_scale=_min_scale_of(c),
+                   bins=bins, percentile=c.detail.get(OBSERVER_PERCENTILE_MANUL_OVERRIDE, OBSERVER_PERCENTILE) if method == 'percentile' else OBSERVER_PERCENTILE)
+        found.setdefault(tuple(key.items()), key)
+    if len(found) > 1:
+        raise ValueError('calibrate_arena: the observed configs differ in ' +
+                         ', '.join(k for k in next(iter(found.values())) if len({f[k] for f in found.values()}) > 1) +
+                         '; one arena serves one setting -- use RuntimeCalibrationPass for mixed configs')
+    return next(iter(found.values())) if found else {}
+
+
 @torch.no_grad()
 def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=None, to_device=None, deferred='auto',
                     graphs: bool = False, prefetch: bool = True, trace: list = None):
@@ -539,17 +562,20 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     graph and replays it for every batch (fixed batch shape).  Capture + instantiate
     costs more than it saves at 8-16 batches per phase, so it is off by default; it pays off for long
     calibration sets or when the same graph is reused across calls.
+    The observed configs must agree in range, bits, symmetry, power-of-two, minimum scale and bin / percentile overrides and be per-tensor
+    (`arena_settings`); asymmetric 'kl' raises PermissionError as upstream, asymmetric 'mse' and more than 12287 KL bins raise ValueError --
+    all before the first batch.
     to_device: a callable applied to every batch, or 'ring' for host tensors staged through the device's persistent DeviceBatchRing.
     trace: a list that receives (phase, batch index, host time, CUDA event, thread CPU time) before every batch and at the end of a phase --
     bench.py's e2e uses it to say whether a slow calibration was slow on the host or on the device, and where."""
     import time
     from .calibration import ArenaCalibrator, is_dense
     cfgs = executor.observed_configs()
+    if graphs and method == 'percentile': raise ValueError('graphs=True needs static statistics buffers; the percentile observer keeps one row per batch')
+    dev = next(executor.model.parameters()).device
+    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group, **arena_settings(cfgs, method))
     for c in cfgs: c.observer_algorithm = method
     if iter(batches) is batches: batches = list(batches)                  # a one-shot iterator would leave phase 2 without data
-    dev = next(executor.model.parameters()).device
-    if graphs and method == 'percentile': raise ValueError('graphs=True needs static statistics buffers; the percentile observer keeps one row per batch')
-    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group)
     static_in = None
     mutated = None                                                        # slots whose tensors are overwritten later in the forward
     phase = 0

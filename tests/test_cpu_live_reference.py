@@ -3,6 +3,7 @@ container; skipped elsewhere -- the committed fixtures in tests/golden/ are what
 generated at run time from a seed: a fixed default keeps the suite deterministic, `PPQ_FUZZ_SEED=random` (or a number) draws a fresh
 one -- 26 different seeds ran clean when this was written -- so the oracle cannot be fitted to a fixed vector set.
 CPU only: reference CPU / torch path (USING_CUDA_KERNEL = False) against oracle/."""
+import math
 import os
 import sys
 import time
@@ -183,3 +184,65 @@ def test_observers_end_to_end(ref, oracle, seed):
         so = [oracle.minmax_to_scale_offset(float(a), float(b), -128, 127, True) for a, b in zip(lo, hi)]
         assert np.array_equal(np.float32([s for s, _ in so]), cfg.scale.numpy().reshape(-1)), (seed, axis)
         assert np.array_equal(np.float32([o for _, o in so]), cfg.offset.numpy().reshape(-1)), (seed, axis)
+
+
+def test_search_configs_vs_reference(ref, oracle, seed, monkeypatch):
+    """The oracle is the expected value of tests/test_gpu_calibration_configs.py for every calibration config, so it is pinned on the real
+    searches for each: power-of-two, 4-bit sym / asym, OBSERVER_MIN_SCALE_MANUL_OVERRIDE, OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE, the MSE
+    interval, zero and constant ranges."""
+    import ppq.quantization.observer.range as rng
+    from ppq.lib import LinearQuantizationConfig
+    from ppq.quantization.observer.range import TorchHistObserver, TorchMSEObserver, minmax_to_scale_offset
+    r = np.random.RandomState(seed + 4)
+
+    def config(sym, bits_, pow2, min_scale=None, kl_bins=None, algo='minmax'):
+        qmin, qmax = (-(1 << (bits_ - 1)), (1 << (bits_ - 1)) - 1) if sym else (0, (1 << bits_) - 1)
+        cfg = LinearQuantizationConfig(symmetrical=sym, quant_min=qmin, quant_max=qmax, num_of_bits=bits_, power_of_2=pow2, calibration=algo)
+        if min_scale is not None: cfg.detail['OBSERVER_MIN_SCALE_MANUL_OVERRIDE'] = min_scale
+        if kl_bins is not None: cfg.detail['OBSERVER_KL_HIST_BINS_MANUL_OVERRIDE'] = kl_bins
+        return cfg, qmin, qmax
+
+    # minmax_to_scale_offset: zero, constant and tiny ranges, powers of two at the minimum scale
+    ranges = [(0.0, 0.0), (0.7, 0.7), (-0.7, -0.7), (-1e-12, 2e-12), (-127.5, 127.5), (0.0, 255.0 * 2 ** -20)]
+    ranges += [(float(np.float32(-abs(a))), float(np.float32(abs(b)))) for a, b in (2.0 ** r.uniform(-30, 30, size=(40, 2)))]
+    for lo, hi in ranges:
+        for sym in (True, False):
+            for bits_ in (4, 8):
+                for pow2 in (False, True):
+                    for ms in (None, 1e-3, 2.0 ** -20, math.nextafter(2.0 ** -20, 1.0)):
+                        cfg, qmin, qmax = config(sym, bits_, pow2, ms)
+                        want = minmax_to_scale_offset(lo, hi, cfg)
+                        got = oracle.minmax_to_scale_offset(lo, hi, qmin, qmax, sym, pow2, 1e-8 if ms is None else ms)
+                        assert (float(got[0]), float(got[1])) == (float(want[0]), float(want[1])), (seed, lo, hi, sym, bits_, pow2, ms)
+    # KL: bin override, 4-bit, power of two, minimum scale, flat (constant data) and single-bin (zero range) histograms
+    for bins in (1024, 2048):
+        hists = [r.poisson(np.linspace(300, 0.01, bins)).astype(np.int64), np.full(bins, 5, np.int64), np.zeros(bins, np.int64)]
+        hists[2][0] = 10 ** 5
+        for hist in hists:
+            for bits_ in (4, 8):
+                for pow2, ms, hs in ((False, None, 1e-3), (True, None, 1e-3), (True, None, 2.0 ** -12 * 3), (False, 0.05, 1e-3), (True, 2.0 ** -20, 0.0)):
+                    cfg, _, _ = config(True, bits_, pow2, ms, kl_bins=bins, algo='kl')
+                    ob = TorchHistObserver(watch_on=None, quant_cfg=cfg)
+                    assert ob._hist_bins == bins
+                    want = ob.hist_to_scale_offset(histogram=torch.tensor(hist.astype(np.int32)), hist_bins=bins, hist_scale=hs, config=cfg)
+                    got = oracle.kl_search(hist, hs, bits_, pow2, 1e-8 if ms is None else ms)
+                    assert (float(got[0]), float(got[1])) == (float(want[0]), float(want[1])), (seed, bins, bits_, pow2, ms, hs)
+    # MSE: 4-bit, asym / sym, interval, power of two, minimum scale, zero and constant ranges
+    bins = 512
+    for it in range(3):
+        hist = r.poisson(np.linspace(50, 0.05, bins)).astype(np.int64)
+        if it == 1: hist = np.full(bins, 3, np.int64)
+        if it == 2: hist = np.zeros(bins, np.int64); hist[bins // 4] = 77
+        for sym in (True, False):
+            for bits_ in (4, 8):
+                for interval in (1, 8, 16):
+                    for pow2, ms, (lo, hi) in ((False, None, (-3.0, 5.0)), (True, None, (-0.05, 5.0)), (False, 2.0 ** -20, (0.0, 0.0)),
+                                               (True, 1e-3, (0.7, 0.7)), (False, None, (0.4, 2.0))):
+                        cfg, qmin, qmax = config(sym, bits_, pow2, ms, algo='mse')
+                        monkeypatch.setattr(rng, 'OBSERVER_MSE_COMPUTE_INTERVAL', interval)
+                        ob = TorchMSEObserver(watch_on=None, quant_cfg=cfg)
+                        ob._min, ob._max = lo, hi
+                        hs = (max(abs(hi), abs(lo)) if sym else (hi - lo)) / bins
+                        want = ob.hist_to_scale_offset(histogram=torch.tensor(hist.astype(np.int32)), hist_bins=bins, hist_scale=hs, config=cfg)
+                        got = oracle.mse_search(hist, hs, lo, qmin, qmax, sym, pow2, interval, oracle.mse_loss_python_twin, 1e-8 if ms is None else ms)
+                        assert (np.float32(got[0]), float(got[1])) == (np.float32(want[0]), float(want[1])), (seed, it, sym, bits_, interval, pow2, ms, lo, hi)
