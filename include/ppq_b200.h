@@ -151,7 +151,9 @@ PPQ_B200_API int ppq_b200_isotone_t(const float *x, int64_t n, float *out4, void
 /* ---- multi-tensor collectors (one launch over a table of tensors; the H100-native calibration path) ---------
  * A descriptor lives in DEVICE memory.  `slot` selects the statistics slot in the arena:
  *   minmax arena: float[2 * slots]  ({min, max} per slot);   hist arena: int32[slots * bins];
- *   hist_scale arena: float[slots]. */
+ *   hist_scale arena: float[slots].
+ * Both keep a prefix of the table's sizes in shared memory ((count + 1) x 8 bytes next to a 64 KB staging ring and, for the histogram,
+ * (bins + 1) x 4 bytes of private counters); a table that does not fit the device's shared memory per block is rejected. */
 typedef struct {
     const float *x;      /* device pointer to the tensor */
     int64_t      n;      /* elements */

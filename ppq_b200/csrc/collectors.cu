@@ -7,8 +7,9 @@
 //   ppq_b200_histogram_c            replaces Histogram_C            (sort.cu:167-218)
 //   ppq_b200_multi_*                one launch over a table of tensors (the calibration arena path, DESIGN.md)
 //
-// All of them read each element exactly once (4 B/element algorithmic traffic) with 128-bit streaming loads, four per
-// thread in flight.  Histograms are privatised per CTA in shared memory (bins x int32, 16 KB for the KL observer's 4096
+// All of them read each element exactly once (4 B/element algorithmic traffic): the single-tensor collectors with 128-bit streaming
+// loads, the multi-tensor ones through a cp.async.bulk ring in shared memory (multi_stream_kernel).  Histograms are privatised per
+// CTA in shared memory (bins x int32, 16 KB for the KL observer's 4096
 // bins) and counted with an unconditional red.shared.add into `bins + 1` slots (the extra one is a trash slot for dropped
 // samples; ptxas emits ATOMS.POPC.INC, which aggregates same-address lanes in hardware, so the post-ReLU pile-up in bin 0 is
 // not a hot spot); only non-empty bins are flushed to the caller's global histogram with red.global.add.
@@ -108,24 +109,6 @@ minmax_t_kernel(const float *__restrict__ x, int64_t n, float *__restrict__ minm
     stream_elements(x, n, (int64_t)blockIdx.x * kThreads + threadIdx.x, (int64_t)gridDim.x * kThreads,
                     [&](float v) { mm.add(v); });
     block_reduce_publish(mm, minmax, minmax + 1);
-}
-
-// One tensor per descriptor, work item = (tensor, chunk of `chunk` elements); blockIdx.x walks the items.
-__global__ void __launch_bounds__(kThreads)
-multi_minmax_t_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, int64_t chunk, int chunks_per_tensor,
-                      float *__restrict__ arena) {
-    const int64_t items = (int64_t)count * chunks_per_tensor;
-    for (int64_t item = blockIdx.x; item < items; item += gridDim.x) {
-        const int t = (int)(item / chunks_per_tensor);
-        const int64_t c = item - (int64_t)t * chunks_per_tensor;
-        const ppq_b200_tensor_desc d = descs[t];
-        const int64_t begin = c * chunk;
-        if (begin >= d.n) continue;                                    // uniform per CTA
-        const int64_t len = (d.n - begin) < chunk ? (d.n - begin) : chunk;
-        MinMax mm;
-        stream_elements(d.x + begin, len, threadIdx.x, kThreads, [&](float v) { mm.add(v); });
-        block_reduce_publish(mm, arena + 2 * (int64_t)d.slot, arena + 2 * (int64_t)d.slot + 1);
-    }
 }
 
 // Per channel: tensor = rows x epc, channel(row) = row % C.  One warp per (row, chunk) work item.
@@ -320,41 +303,172 @@ histogram_dscale_kernel(const float *__restrict__ x, int64_t n, const float *__r
     hist_flush<VARIANT>(sh, bins, hist);
 }
 
-template <int VARIANT>
-__global__ void __launch_bounds__(kHistThreads)
-multi_histogram_t_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count,
-                         const float *__restrict__ hist_scale_arena, int clip, int bins, int32_t *__restrict__ hist_arena) {
-    // Each CTA owns one contiguous span of the concatenation of all tensors, so the private bins are zeroed / flushed
-    // (#CTAs + #tensors) times in total instead of once per fixed-size chunk.
-    extern __shared__ int sh[];
-    int64_t *prefix = reinterpret_cast<int64_t *>(sh + ((bins + 1 + 1) & ~1));       // [count + 1], 8-byte aligned
+// ---- multi-tensor collectors: one streaming engine ------------------------------------------------------------------------
+// Each CTA owns one contiguous span of the concatenation of all tensors (cut points inside a tensor rounded up to a multiple of 4
+// elements, the same way by both neighbours), so per-tensor state is set up and published (#CTAs + #tensors) times per launch.
+// Warp-specialised CTA: one producer lane walks the CTA's pieces (tensor t, elements [a, b)) and issues 1-D cp.async.bulk copies of
+// their 16-byte-aligned bodies into a ring of kRingStages tiles (full / empty mbarriers); the consumer warps walk the same pieces,
+// apply Op to every element of each tile from shared memory, and handle the (at most 3 + 3) unaligned head / tail elements of a piece
+// with plain loads.  Copies keep flowing while the consumers bin, flush or wait at a piece boundary.
+constexpr int kRingConsumers = 512;                  // 16 consumer warps
+constexpr int kRingThreads = kRingConsumers + 32;    // + the producer warp
+constexpr int kRingTileVec = 1024;                   // float4 per tile (16 KB): two per consumer thread
+constexpr int kRingStages = 4;                       // 64 KB of tiles per CTA
+constexpr int kRingBarId = 1;                        // named barrier of the consumer warps (0 is __syncthreads)
+
+__device__ __forceinline__ uint32_t smem_addr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void ring_wait(uint64_t *bar, uint32_t parity) {
+    asm volatile("{\n.reg .pred p;\nWAIT_%=:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}\n"
+                 ::"r"(smem_addr(bar)), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync %0, %1;" ::"n"(kRingBarId), "n"(kRingConsumers) : "memory"); }
+
+// Per-tensor min/max: registers per (CTA, tensor), one publish per visit.
+struct MinMaxOp {
+    struct Args { float *arena; };
+    static size_t smem_bytes(int) { return 2 * 2 * (kRingConsumers / 32) * sizeof(float); }
+    Args g; float *s_lo; MinMax mm; int visit;
+    __device__ __forceinline__ MinMaxOp(const Args &a, void *smem) : g(a), s_lo(reinterpret_cast<float *>(smem)), visit(0) {}
+    __device__ __forceinline__ void begin(const ppq_b200_tensor_desc &) { mm = MinMax(); }
+    __device__ __forceinline__ void add(float v) { mm.add(v); }
+    __device__ __forceinline__ void add4(const float4 &v) { mm.add4(v); }
+    __device__ __forceinline__ void end(const ppq_b200_tensor_desc &d) {
+        // two alternating staging buffers: warp 0 has read buffer v before anyone passes the barrier of visit v + 1
+        float *lo = s_lo + (visit & 1) * 2 * (kRingConsumers / 32), *hi = lo + kRingConsumers / 32;
+        visit++;
+        const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+        mm.warp_reduce();
+        if (l == 0) { lo[w] = mm.lo; hi[w] = mm.hi; }
+        consumers_sync();
+        if (w == 0) {
+            MinMax t;
+            if (l < kRingConsumers / 32) { t.lo = lo[l]; t.hi = hi[l]; }
+            t.warp_reduce();
+            if (l == 0) t.publish(g.arena + 2 * (int64_t)d.slot, g.arena + 2 * (int64_t)d.slot + 1);
+        }
+    }
+};
+
+// Per-tensor symmetric histogram with device-side hist_scale: CTA-private bins (+ trash slot) in shared memory, non-empty bins flushed
+// with red.global.add once per visit.
+struct HistOp {
+    struct Args { const float *hist_scale_arena; int32_t *hist_arena; int bins, clip; };
+    static size_t smem_bytes(int bins) { return (size_t)(bins + 1) * sizeof(int); }
+    Args g; int *sh; SymBin bin; Counter<0> cnt;
+    __device__ __forceinline__ HistOp(const Args &a, void *smem)
+        : g(a), sh(reinterpret_cast<int *>(smem)), bin(1.f, a.bins, a.clip != 0), cnt(sh, nullptr, a.bins) {
+        for (int i = threadIdx.x; i <= g.bins; i += kRingConsumers) sh[i] = 0;
+        consumers_sync();
+    }
+    __device__ __forceinline__ void begin(const ppq_b200_tensor_desc &d) { bin = SymBin(__ldg(g.hist_scale_arena + d.slot), g.bins, g.clip != 0); }
+    __device__ __forceinline__ void add(float v) { cnt.count(bin(v)); }
+    __device__ __forceinline__ void add4(const float4 &v) { const uint4 b = bin.bin4(v); cnt.count(b.x); cnt.count(b.y); cnt.count(b.z); cnt.count(b.w); }
+    __device__ __forceinline__ void end(const ppq_b200_tensor_desc &d) {
+        consumers_sync();                                              // every count of this visit has landed
+        int32_t *gh = g.hist_arena + (int64_t)d.slot * g.bins;
+        for (int i = threadIdx.x; i <= g.bins; i += kRingConsumers) {
+            const int v = sh[i];
+            if (v && i < g.bins) atomicAdd(gh + i, v);
+            sh[i] = 0;
+        }
+        consumers_sync();                                              // zeroed before the next visit counts
+    }
+};
+
+// Shared memory: [ring kRingStages x 16 KB][full, empty mbarriers][prefix int64 x (count + 1)][Op's own]
+__host__ __device__ inline size_t ring_prefix_offset() { return (size_t)kRingStages * kRingTileVec * 16 + 2 * kRingStages * sizeof(uint64_t); }
+__host__ __device__ inline size_t ring_op_offset(int count) { return ring_prefix_offset() + (size_t)(count + 1) * sizeof(int64_t); }
+
+template <class Op>
+__global__ void __launch_bounds__(kRingThreads, 2)
+multi_stream_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, typename Op::Args args) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    float4 *ring = reinterpret_cast<float4 *>(smem);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)kRingStages * kRingTileVec * 16), *empty = full + kRingStages;
+    int64_t *prefix = reinterpret_cast<int64_t *>(smem + ring_prefix_offset());
+    // parallel prefix of the tensor sizes: every thread loads, warp 0 scans 32 contiguous runs
+    for (int t = threadIdx.x; t < count; t += kRingThreads) prefix[t + 1] = descs[t].n;
     if (threadIdx.x == 0) {
+        prefix[0] = 0;
+        for (int s = 0; s < kRingStages; s++) {
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_addr(full + s)));
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(empty + s)), "r"(kRingConsumers / 32));
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int per = (count + 31) / 32, t0 = threadIdx.x * per, t1 = min(count, t0 + per);
         int64_t run = 0;
-        for (int t = 0; t < count; t++) { prefix[t] = run; run += descs[t].n; }
-        prefix[count] = run;
+        for (int t = t0; t < t1; t++) run += prefix[t + 1];
+        int64_t incl = run;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int64_t u = __shfl_up_sync(0xffffffffu, incl, o); if ((int)threadIdx.x >= o) incl += u; }
+        run = incl - run;
+        for (int t = t0; t < t1; t++) { run += prefix[t + 1]; prefix[t + 1] = run; }
     }
     __syncthreads();
     const int64_t total = prefix[count];
     int64_t span = (total + gridDim.x - 1) / gridDim.x;
     span = (span + 3) & ~(int64_t)3;
     const int64_t s0 = (int64_t)blockIdx.x * span, s1 = (s0 + span) < total ? (s0 + span) : total;
-    if (s0 >= total) return;
-    int t = 0;                                                         // first tensor overlapping [s0, s1): binary search
-    { int lo = 0, hi = count - 1; while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (prefix[mid] <= s0) lo = mid; else hi = mid - 1; } t = lo; }
-    for (; t < count && prefix[t] < s1; t++) {
-        const ppq_b200_tensor_desc d = descs[t];
-        int64_t a = s0 - prefix[t]; if (a < 0) a = 0;
-        int64_t b = s1 - prefix[t]; if (b > d.n) b = d.n;
-        a = (a + 3) & ~(int64_t)3; if (a > d.n) a = d.n;               // both neighbours round the shared boundary the same way
-        if (b < d.n) b = (b + 3) & ~(int64_t)3; if (b > d.n) b = d.n;
-        if (b <= a) continue;                                          // uniform per CTA
-        int32_t *gh = hist_arena + (int64_t)d.slot * bins;
-        hist_zero<VARIANT>(sh, bins);
-        Counter<VARIANT> cnt(sh, gh, bins);
-        const SymBin bin(__ldg(hist_scale_arena + d.slot), bins, clip != 0);
-        hist_stream<VARIANT>(d.x + a, b - a, threadIdx.x, kHistThreads, bin, cnt);
-        hist_flush<VARIANT>(sh, bins, gh);
+    if (s0 >= total) return;                                           // uniform per CTA
+    int t_first;                                                       // first tensor overlapping [s0, s1): binary search
+    { int lo = 0, hi = count - 1; while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (prefix[mid] <= s0) lo = mid; else hi = mid - 1; } t_first = lo; }
+
+    // The pieces of this CTA, walked identically by the producer and the consumers.  body = [ia, ia + 4 nv) is 16-byte aligned.
+    auto for_each_piece = [&](auto &&f) {
+        for (int t = t_first; t < count && prefix[t] < s1; t++) {
+            const ppq_b200_tensor_desc d = descs[t];
+            int64_t a = s0 - prefix[t]; if (a < 0) a = 0;
+            int64_t b = s1 - prefix[t]; if (b > d.n) b = d.n;
+            a = (a + 3) & ~(int64_t)3; if (a > d.n) a = d.n;
+            if (b < d.n) b = (b + 3) & ~(int64_t)3; if (b > d.n) b = d.n;
+            if (b <= a) continue;
+            int64_t ia = a + (int64_t)((4u - (uint32_t)((reinterpret_cast<uintptr_t>(d.x + a) >> 2) & 3u)) & 3u);
+            if (ia > b) ia = b;
+            f(d, a, b, ia, (b - ia) >> 2);
+        }
+    };
+    if (threadIdx.x >= kRingConsumers) {
+        if (threadIdx.x == kRingConsumers) {                           // producer: one lane
+            uint32_t k = 0;
+            for_each_piece([&](const ppq_b200_tensor_desc &d, int64_t, int64_t, int64_t ia, int64_t nv) {
+                const float4 *src = reinterpret_cast<const float4 *>(d.x + ia);
+                for (int64_t v0 = 0; v0 < nv; v0 += kRingTileVec, k++) {
+                    const uint32_t s = k % kRingStages, bytes = (uint32_t)((nv - v0) < kRingTileVec ? (nv - v0) : kRingTileVec) * 16u;
+                    if (k >= kRingStages) ring_wait(empty + s, ((k / kRingStages) - 1) & 1);
+                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(full + s)), "r"(bytes) : "memory");
+                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                                 ::"r"(smem_addr(ring + s * kRingTileVec)), "l"(src + v0), "r"(bytes), "r"(smem_addr(full + s)) : "memory");
+                }
+            });
+        }
+        return;
     }
+    Op op(args, smem + ring_op_offset(count));
+    uint32_t k = 0;
+    for_each_piece([&](const ppq_b200_tensor_desc &d, int64_t a, int64_t b, int64_t ia, int64_t nv) {
+        op.begin(d);
+        const int64_t ib = ia + 4 * nv;                                // ragged head [a, ia) and tail [ib, b): at most 3 + 3 elements
+        const int i = (int)threadIdx.x, head = (int)(ia - a);
+        if (i < head) op.add(ld_stream1(d.x + a + i));
+        else if (i < head + (int)(b - ib)) op.add(ld_stream1(d.x + ib + (i - head)));
+        for (int64_t v0 = 0; v0 < nv; v0 += kRingTileVec, k++) {
+            const uint32_t s = k % kRingStages;
+            const int cnt = (int)((nv - v0) < kRingTileVec ? (nv - v0) : kRingTileVec);
+            ring_wait(full + s, (k / kRingStages) & 1);
+            const float4 *tile = ring + s * kRingTileVec;
+#pragma unroll
+            for (int j = 0; j < kRingTileVec / kRingConsumers; j++) {
+                const int vi = i + j * kRingConsumers;
+                if (vi < cnt) op.add4(tile[vi]);
+            }
+            __syncwarp();
+            if ((i & 31) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + s)) : "memory");
+        }
+        op.end(d);
+    });
 }
 
 // Per-channel histogram: rows x epc, hist[c][bins].  One CTA per (row, chunk); smem holds that row's private bins.
@@ -414,6 +528,31 @@ static int launch_hist(const float *x, int64_t n, const BinParams &bin, int64_t 
     // default: two 1024-thread CTAs per SM (32 registers per thread), 2 loads in flight per thread
     default: histogram_kernel<0, Bin, 2, kHistThreads, 2><<<grid * 2 > sm_count() * 2 ? sm_count() * 2 : grid * 2, kHistThreads, smem, st>>>(x, n, bin, hist); break;
     }
+    return (int)cudaGetLastError();
+}
+
+// Two CTAs per SM when the ring, the prefix and the Op's shared memory allow it; each CTA should own >= 64 Ki elements before it pays
+// for its per-tensor set-up and publishes.  Rejects tables whose shared memory exceeds the device's opt-in limit.
+template <class Op>
+static int launch_multi_stream(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, const typename Op::Args &args, int op_param,
+                               cudaStream_t st) {
+    const size_t smem = ring_op_offset(count) + Op::smem_bytes(op_param);
+    int dev = 0, limit = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess)
+        return (int)cudaGetLastError();
+    if (smem > (size_t)limit) return (int)cudaErrorInvalidValue;
+    // the > 48 KB opt-in is per device, not per process: set it on every launch
+    if (cudaFuncSetAttribute(multi_stream_kernel<Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return (int)cudaGetLastError();
+    int resident = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, multi_stream_kernel<Op>, kRingThreads, smem) != cudaSuccess)
+        return (int)cudaGetLastError();
+    if (resident < 1) resident = 1;
+    if (resident > 2) resident = 2;
+    int64_t g = ((int64_t)count * max_n + 65535) / 65536;
+    if (g > (int64_t)sm_count() * resident) g = (int64_t)sm_count() * resident;
+    if (g < 1) g = 1;
+    multi_stream_kernel<Op><<<(int)g, kRingThreads, smem, st>>>(descs, count, args);
     return (int)cudaGetLastError();
 }
 
@@ -490,27 +629,14 @@ int ppq_b200_histogram_c(const float *x, int64_t n, int64_t epc, int C, float hi
 
 int ppq_b200_multi_minmax_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float *minmax_arena, void *stream) {
     if (count <= 0 || max_n <= 0 || !descs || !minmax_arena) return (int)cudaErrorInvalidValue;
-    const int64_t chunk = 65536;
-    const int64_t cpt = (max_n + chunk - 1) / chunk;
-    if (cpt > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-    const int64_t items = (int64_t)count * cpt;
-    const int grid = (int)(items < (int64_t)sm_count() * 8 ? items : (int64_t)sm_count() * 8);
-    multi_minmax_t_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(descs, count, chunk, (int)cpt, minmax_arena);
-    return (int)cudaGetLastError();
+    return launch_multi_stream<MinMaxOp>(descs, count, max_n, MinMaxOp::Args{minmax_arena}, 0, (cudaStream_t)stream);
 }
 
 int ppq_b200_multi_histogram_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, const float *hist_scale_arena,
                                int clip_outliers, int32_t *hist_arena, int64_t bins, void *stream) {
     if (count <= 0 || max_n <= 0 || !descs || !hist_scale_arena || !hist_arena || bins <= 0 || bins > kMaxSmemBins) return (int)cudaErrorInvalidValue;
-    const size_t smem = (size_t)((bins + 2) & ~1) * sizeof(int) + (size_t)(count + 1) * sizeof(int64_t);
-    if (smem > 48 * 1024) return (int)cudaErrorInvalidValue;
-    // grid: one CTA per SM, fewer when the whole job is small (each CTA should own >= 64 Ki elements before paying for a flush)
-    int64_t g = ((int64_t)count * max_n + 65535) / 65536;
-    if (g > sm_count()) g = sm_count();
-    if (g < 1) g = 1;
-    multi_histogram_t_kernel<0><<<(int)g, kHistThreads, smem, (cudaStream_t)stream>>>(descs, count, hist_scale_arena, clip_outliers, (int)bins,
-                                                                                      hist_arena);
-    return (int)cudaGetLastError();
+    return launch_multi_stream<HistOp>(descs, count, max_n, HistOp::Args{hist_scale_arena, hist_arena, (int)bins, clip_outliers}, (int)bins,
+                                       (cudaStream_t)stream);
 }
 
 }  // extern "C"
