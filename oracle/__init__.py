@@ -22,6 +22,9 @@ Pinning status (tests/test_oracle_pinning.py):
   the reference has no CPU implementation and no test -> pinned on the GPU against the reference's own
   CUDA kernels compiled for sm_90a (oracle/_ref/PPQ_Cuda_Impls_ref.so, tests/test_gpu_vs_reference_cuda.py);
   fixtures produced there are committed under tests/golden/ref_cuda_*.npz once available.
+  Training-pass kernels (LSQ / float backward, TensorClip, RoundingLoss): pinned on the CPU against the torch formulas of the reference's
+  own test plus hand-worked answers (tests/test_cpu_training_oracle.py), and on the GPU against the reference's recorded CUDA calls
+  (tests/test_gpu_training_kernels.py).
 """
 import ctypes
 import math
@@ -91,6 +94,14 @@ def lib():
         L.ora_minmax_t.argtypes = [_P, _I64, _P, _P]
         L.ora_minmax_c.argtypes = [_P, _I64, _I64, _I32, _P, _P]
         L.ora_quantile_t.argtypes = [_P, _I64, _F, _P]
+        L.ora_linear_quant_backward.restype = _F
+        L.ora_linear_quant_backward.argtypes = [_P, _P, _I64, _I64, _I32, _I32, _P, _P, _I32, _I32, _I32, _P, _P]
+        L.ora_float_quant_backward.restype = _F
+        L.ora_float_quant_backward.argtypes = [_P, _P, _I64, _I64, _I32, _I32, _P, _P, _I32, _I32, _F, _F, _I32, _P, _P]
+        L.ora_tensor_clip.argtypes = [_P, _P, _P, _I64, _I64, _I32, _I32, _P]
+        L.ora_rounding_loss.restype = _F
+        L.ora_rounding_loss.argtypes = [_P, _I64, _I64, _I32, _I32, _P, _P, _I32, _I32, _I32, _P]
+        L.ora_rounding_loss_backward.argtypes = [_P, _F, _I64, _I64, _I32, _I32, _P, _P, _I32, _I32, _I32, _P]
         _lib = L
     return _lib
 
@@ -164,6 +175,61 @@ def float_quant_c(x, scale, offset, axis, E=4, M=3, cmin=-448.0, cmax=448.0, mod
     lib().ora_float_quant_c(x.ctypes.data, y.ctypes.data, x.size, epc, C, s.ctypes.data, o.ctypes.data,
                             E, M, float(cmin), float(cmax), int(mode))
     return y
+
+
+# ---- training-pass kernels -------------------------------------------------------------------------
+def _train_geometry(x, scale, offset, axis):
+    """(scale, offset, epc, C, per_channel) as fp32 arrays; axis=None means per tensor (scale[0], offset[0])."""
+    s = _f32(scale).reshape(-1); o = _f32(offset).reshape(-1)
+    if axis is None:
+        return s[:1].copy(), o[:1].copy(), max(x.size, 1), 1, 0
+    epc, C = channel_geometry(x.shape, axis)
+    assert s.size == C and o.size == C
+    return s, o, epc, C, 1
+
+
+def linear_quant_backward(x, dy, scale, offset, qmin, qmax, mode=0, axis=None):
+    """QuantizeTensor_LT_B (axis=None) / _LC_B: (grad_x, per-element fp32 partials of grad_s, factor applied to each block sum)."""
+    x = _f32(x); dy = _f32(dy); gx = np.empty_like(x); p = np.empty_like(x)
+    s, o, epc, C, pc = _train_geometry(x, scale, offset, axis)
+    f = lib().ora_linear_quant_backward(x.ctypes.data, dy.ctypes.data, x.size, epc, C, pc, s.ctypes.data, o.ctypes.data,
+                                        int(qmin), int(qmax), int(mode), gx.ctypes.data, p.ctypes.data)
+    return gx, p, np.float32(f)
+
+
+def float_quant_backward(x, dy, scale, offset, E, M, cmin, cmax, mode=0, axis=None):
+    """QuantizeTensor_FT_B (axis=None) / _FC_B: (grad_x, per-element fp32 partials of grad_s, divisor of each block sum)."""
+    x = _f32(x); dy = _f32(dy); gx = np.empty_like(x); p = np.empty_like(x)
+    s, o, epc, C, pc = _train_geometry(x, scale, offset, axis)
+    d = lib().ora_float_quant_backward(x.ctypes.data, dy.ctypes.data, x.size, epc, C, pc, s.ctypes.data, o.ctypes.data,
+                                       int(E), int(M), float(np.float32(cmin)), float(np.float32(cmax)), int(mode), gx.ctypes.data, p.ctypes.data)
+    return gx, p, np.float32(d)
+
+
+def tensor_clip(value, reference, limit, axis=None):
+    """TensorClip_T (axis=None) / _C."""
+    v = _f32(value); r = _f32(reference); out = np.empty_like(v)
+    lim, _, epc, C, pc = _train_geometry(v, limit, limit, axis)
+    lib().ora_tensor_clip(v.ctypes.data, r.ctypes.data, lim.ctypes.data, v.size, epc, C, pc, out.ctypes.data)
+    return out
+
+
+def rounding_loss(x, scale, offset, qmin, qmax, mode=0, axis=None):
+    """RoundingLoss_LT (axis=None) / _LC: (per-element fp32 |deq - v| terms, divisor of each block sum)."""
+    x = _f32(x); p = np.empty_like(x)
+    s, o, epc, C, pc = _train_geometry(x, scale, offset, axis)
+    d = lib().ora_rounding_loss(x.ctypes.data, x.size, epc, C, pc, s.ctypes.data, o.ctypes.data, int(qmin), int(qmax), int(mode),
+                                p.ctypes.data)
+    return p, np.float32(d)
+
+
+def rounding_loss_backward(x, dy, scale, offset, qmin, qmax, mode=0, axis=None):
+    """RoundingLoss_LT_B (axis=None) / _LC_B; only dy[0] is read."""
+    x = _f32(x); gx = np.empty_like(x)
+    s, o, epc, C, pc = _train_geometry(x, scale, offset, axis)
+    lib().ora_rounding_loss_backward(x.ctypes.data, float(_f32(dy).reshape(-1)[0]), x.size, epc, C, pc, s.ctypes.data, o.ctypes.data,
+                                     int(qmin), int(qmax), int(mode), gx.ctypes.data)
+    return gx
 
 
 # ---- collectors ------------------------------------------------------------------------------------
