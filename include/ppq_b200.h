@@ -9,7 +9,8 @@
  * installs it (CUDA_COMPLIER.__CUDA_EXTENTION__ = ppq_b200.extension()).
  *
  * Conventions (all functions unless stated otherwise)
- *   - plain pointers and sizes, no torch types; all tensors fp32, flat, contiguous, DEVICE memory;
+ *   - plain pointers and sizes, no torch types; all tensors fp32 (the `_dt` entries also take fp16 / bf16 values),
+ *     flat, contiguous, DEVICE memory;
  *   - `scale` / `offset` are DEVICE pointers (1 element per-tensor, C elements per-channel), exactly what the
  *     reference passes (scale/offset tensors live on the executor device);
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream);
@@ -35,6 +36,14 @@ extern "C" {
 #else
 #define PPQ_B200_API
 #endif
+
+/* ---- element types ------------------------------------------------------------------------------ */
+/* The `_dt` entries take `const void *x` plus one of these codes.  For fp16 / bf16 every statistic equals the fp32 one on the exact
+ * upcast x.float(); a fake-quantised output has the input's type and holds the fp32 result rounded once to nearest even.
+ * Scales, offsets and statistics stay fp32.  Any other code returns cudaErrorInvalidValue before a launch. */
+#define PPQ_B200_F32  0
+#define PPQ_B200_F16  1
+#define PPQ_B200_BF16 2
 
 /* ---- library ----------------------------------------------------------------------------------- */
 PPQ_B200_API int         ppq_b200_abi_version(void);              /* bumps when a signature changes */
@@ -62,6 +71,19 @@ PPQ_B200_API int ppq_b200_linear_quant_t_toint(const float *x, void *q, int out_
 PPQ_B200_API int ppq_b200_linear_quant_c_toint(const float *x, void *q, int out_bits, int64_t n, int64_t epc, int C,
                                                const float *scale, const float *offset,
                                                int qmin, int qmax, int rounding, void *stream);
+/* The four entries above for an input of element type `dtype` (PPQ_B200_F32 / _F16 / _BF16); `y` has the input's type. */
+PPQ_B200_API int ppq_b200_linear_quant_t_dt(const void *x, int dtype, void *y, int64_t n,
+                                            const float *scale, const float *offset,
+                                            int qmin, int qmax, int rounding, void *stream);
+PPQ_B200_API int ppq_b200_linear_quant_c_dt(const void *x, int dtype, void *y, int64_t n, int64_t epc, int C,
+                                            const float *scale, const float *offset,
+                                            int qmin, int qmax, int rounding, void *stream);
+PPQ_B200_API int ppq_b200_linear_quant_t_toint_dt(const void *x, int dtype, void *q, int out_bits, int64_t n,
+                                                  const float *scale, const float *offset,
+                                                  int qmin, int qmax, int rounding, void *stream);
+PPQ_B200_API int ppq_b200_linear_quant_c_toint_dt(const void *x, int dtype, void *q, int out_bits, int64_t n, int64_t epc, int C,
+                                                  const float *scale, const float *offset,
+                                                  int qmin, int qmax, int rounding, void *stream);
 
 /* Every per-channel weight of a network in ONE launch (the executor re-quantises all Conv/Gemm weights on every forward until
  * they are baked: ppq/executor/torch.py:516-518; ParameterBakingPass, optim/baking.py:34-47).  Descriptors in DEVICE memory. */
@@ -105,6 +127,15 @@ PPQ_B200_API int ppq_b200_float_quant_c(const float *x, float *y, int64_t n, int
                                         const float *scale, const float *offset,
                                         int exponent, int mantissa, float clip_min, float clip_max,
                                         int rounding, void *stream);
+/* The two entries above for an input of element type `dtype`; `y` has the input's type. */
+PPQ_B200_API int ppq_b200_float_quant_t_dt(const void *x, int dtype, void *y, int64_t n,
+                                           const float *scale, const float *offset,
+                                           int exponent, int mantissa, float clip_min, float clip_max,
+                                           int rounding, void *stream);
+PPQ_B200_API int ppq_b200_float_quant_c_dt(const void *x, int dtype, void *y, int64_t n, int64_t epc, int C,
+                                           const float *scale, const float *offset,
+                                           int exponent, int mantissa, float clip_min, float clip_max,
+                                           int rounding, void *stream);
 
 /* ---- calibration collectors ---------------------------------------------------------------------- */
 /* Fused single-pass min+max.  Replaces the two torch reductions of TorchMinMaxObserver.observe,
@@ -132,6 +163,14 @@ PPQ_B200_API int ppq_b200_histogram_c(const float *x, int64_t n, int64_t epc, in
  * ppq_b200_hist_scale_from_minmax), so phase 2 of the calibration needs no host round-trip. */
 PPQ_B200_API int ppq_b200_histogram_t_dscale(const float *x, int64_t n, const float *hist_scale_dev, int clip_outliers,
                                              int32_t *hist, int64_t bins, void *stream);
+/* min/max and the two histograms above for an input of element type `dtype`: the same statistics as on the fp32 upcast. */
+PPQ_B200_API int ppq_b200_minmax_t_dt(const void *x, int dtype, int64_t n, float *minmax, void *stream);
+PPQ_B200_API int ppq_b200_minmax_c_dt(const void *x, int dtype, int64_t n, int64_t epc, int C,
+                                      float *mins, float *maxs, void *stream);
+PPQ_B200_API int ppq_b200_histogram_asym_t_dt(const void *x, int dtype, int64_t n, float vmin, float vmax, int clip_outliers,
+                                              int32_t *hist, int64_t bins, void *stream);
+PPQ_B200_API int ppq_b200_histogram_t_dscale_dt(const void *x, int dtype, int64_t n, const float *hist_scale_dev, int clip_outliers,
+                                                int32_t *hist, int64_t bins, void *stream);
 
 /* replaces Quantile_T, sort.cu:6-20, 42-59 (ffi.py:171-176): out[0] = sorted[clip(rn(n*q))], out[1] = sorted[clip(rn(n*(1-q)))],
  * found by an exact radix select on the order-preserving key (no clone, no full sort; same element bit for bit): two streaming passes
@@ -145,6 +184,9 @@ PPQ_B200_API int ppq_b200_quantile_t(const float *x, int64_t n, float q, float *
 /* the same with a one-slot `guess` buffer (see ppq_b200_multi_quantile_t): consecutive calls on batches of one activation -- what
  * TorchPercentileObserver.observe does (range.py:338-349) -- read the tensor once when the previous call's thresholds still hold. */
 PPQ_B200_API int ppq_b200_quantile_t_guess(const float *x, int64_t n, float q, float *out2, void *workspace, uint32_t *guess, void *stream);
+/* both of the above for an input of element type `dtype` (guess may be NULL): the selected values are the exact fp32 upcasts. */
+PPQ_B200_API int ppq_b200_quantile_t_dt(const void *x, int dtype, int64_t n, float q, float *out2, void *workspace, uint32_t *guess,
+                                        void *stream);
 /* replaces Isotone_T, sort.cu:23-40, 61-73: out4 = {sorted[n-1], sorted[n-2], sorted[0], sorted[1]} (same workspace). */
 PPQ_B200_API int ppq_b200_isotone_t(const float *x, int64_t n, float *out4, void *workspace, void *stream);
 

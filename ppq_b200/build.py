@@ -30,7 +30,7 @@ NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-
               '--expt-relaxed-constexpr', '--expt-extended-lambda',
               '-Xcompiler', '-fPIC,-fvisibility=hidden,-ffp-contract=off,-Wall', '-I', INCLUDE]
 CU_SOURCES = ['fakequant.cu', 'fakequant_tma.cu', 'collectors.cu', 'search.cu', 'select.cu', 'train.cu', 'host.cc']
-HEADERS = ['common.cuh', 'ops.cuh', 'variants.h', os.path.join(INCLUDE, 'ppq_b200.h')]
+HEADERS = ['common.cuh', 'ops.cuh', 'half.cuh', 'variants.h', os.path.join(INCLUDE, 'ppq_b200.h')]
 
 
 def _newest(paths):

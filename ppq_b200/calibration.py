@@ -464,6 +464,9 @@ class MultiWeightQuantizer:
         self.ext = extension()
         self.quant_min, self.quant_max, self.rounding = quant_min, quant_max, rounding
         self.per_tensor = channel_axis is None
+        # the descriptor table carries raw pointers and the table kernels read and write fp32: any other dtype must never reach them
+        bad = sorted({str(t.dtype) for t in list(weights) + list(scales) + list(offsets) if t.dtype != torch.float32})
+        if bad: raise TypeError(f'MultiWeightQuantizer takes fp32 weights, scales and offsets only, got {", ".join(bad)}.')
 
         def rows_in_storage_order(w):
             # axis-0 channels of a dense tensor whose dim 0 is outermost in memory (NCHW or channels_last weights): the storage already is [C, epc]

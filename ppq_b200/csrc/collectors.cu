@@ -14,6 +14,7 @@
 // samples; ptxas emits ATOMS.POPC.INC, which aggregates same-address lanes in hardware, so the post-ReLU pile-up in bin 0 is
 // not a hot spot); only non-empty bins are flushed to the caller's global histogram with red.global.add.
 #include "common.cuh"
+#include "half.cuh"
 #include "../../include/ppq_b200.h"
 #include "variants.h"
 #include <cooperative_groups.h>
@@ -94,6 +95,34 @@ __device__ __forceinline__ void stream_elements(const float *__restrict__ x, int
     }
 }
 
+// The same for fp16 / bf16: 16-byte loads of 8 elements converted to fp32 in registers; the <= 7 elements before the first 16-byte
+// boundary and the <= 7 after the last whole vector go one per thread to the first threads of the group.
+template <class T, class F, std::enable_if_t<is_half_t<T>::value, int> = 0>
+__device__ __forceinline__ void stream_elements(const T *__restrict__ x, int64_t n, int64_t first, int64_t stride, F &&f) {
+    const int64_t head = min(n, head_elems(x));
+    const int64_t nv = (n - head) >> 3, tail0 = head + (nv << 3);
+    const uint4 *x8 = reinterpret_cast<const uint4 *>(x + head);
+    constexpr int64_t kSeg = 32 * kUnroll;
+    const int64_t lane = first & 31, warp = first >> 5, warps = stride >> 5;
+    const int64_t segs = (nv + kSeg - 1) / kSeg;
+    for (int64_t sg = warp; sg < segs; sg += warps) {
+        const int64_t base = sg * kSeg + lane;
+        uint4 v[kUnroll];
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) if (base + j * 32 < nv) v[j] = ld_stream_u4(x8 + base + j * 32);
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) {
+            if (base + j * 32 < nv) {
+                float4 a, b;
+                unpack8<T>(v[j], a, b);
+                f(a.x); f(a.y); f(a.z); f(a.w); f(b.x); f(b.y); f(b.z); f(b.w);
+            }
+        }
+    }
+    if (first < head) f(ld_stream1_f(x + first));
+    else if (first - head < n - tail0) f(ld_stream1_f(x + tail0 + (first - head)));
+}
+
 // ---- min / max ------------------------------------------------------------------------------------------------------
 __global__ void minmax_init_kernel(float *mins, float *maxs, int64_t count) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -103,8 +132,9 @@ __global__ void minmax_init_kernel(float *mins, float *maxs, int64_t count) {
     }
 }
 
+template <class T>
 __global__ void __launch_bounds__(kThreads)
-minmax_t_kernel(const float *__restrict__ x, int64_t n, float *__restrict__ minmax) {
+minmax_t_kernel(const T *__restrict__ x, int64_t n, float *__restrict__ minmax) {
     MinMax mm;
     stream_elements(x, n, (int64_t)blockIdx.x * kThreads + threadIdx.x, (int64_t)gridDim.x * kThreads,
                     [&](float v) { mm.add(v); });
@@ -113,8 +143,9 @@ minmax_t_kernel(const float *__restrict__ x, int64_t n, float *__restrict__ minm
 
 // Per channel: tensor = rows x epc, channel(row) = row % C.  One warp per (row, chunk) work item.
 constexpr int kRowChunk = 4096;
+template <class T>
 __global__ void __launch_bounds__(kThreads)
-minmax_c_kernel(const float *__restrict__ x, int64_t rows, int64_t epc, int C, int64_t chunks_per_row,
+minmax_c_kernel(const T *__restrict__ x, int64_t rows, int64_t epc, int C, int64_t chunks_per_row,
                 FastDiv div_chunks, FastDiv div_C, float *__restrict__ mins, float *__restrict__ maxs) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = (int64_t)gridDim.x * (kThreads / 32);
@@ -246,12 +277,51 @@ __device__ __forceinline__ void hist_stream(const float *__restrict__ x, int64_t
     }
 }
 
+// fp16 / bf16: 16-byte loads of 8 elements, same warp-uniform trip counts and trash padding; the <= 7 + 7 unaligned head and tail
+// elements go one per thread to the first threads of the group.
+template <int VARIANT, class Bin, int U = kUnroll, class T, std::enable_if_t<is_half_t<T>::value, int> = 0>
+__device__ __forceinline__ void hist_stream(const T *__restrict__ x, int64_t n, int64_t first, int64_t stride,
+                                            const Bin &bin, Counter<VARIANT> &cnt) {
+    const int64_t head = min(n, head_elems(x));
+    const int64_t nv = (n - head) >> 3, tail0 = head + (nv << 3);
+    const uint4 *x8 = reinterpret_cast<const uint4 *>(x + head);
+    const int64_t warp_first = first - (threadIdx.x & 31);
+    auto count8 = [&](const uint4 &r, bool ok) {
+        float4 a, b;
+        unpack8<T>(r, a, b);
+        const uint4 ba = bin.bin4(a), bb = bin.bin4(b);
+        cnt.count(ok ? ba.x : cnt.trash); cnt.count(ok ? ba.y : cnt.trash); cnt.count(ok ? ba.z : cnt.trash); cnt.count(ok ? ba.w : cnt.trash);
+        cnt.count(ok ? bb.x : cnt.trash); cnt.count(ok ? bb.y : cnt.trash); cnt.count(ok ? bb.z : cnt.trash); cnt.count(ok ? bb.w : cnt.trash);
+    };
+    int64_t i = first;
+    for (; warp_first + (i - first) + 31 + (U - 1) * stride < nv; i += U * stride) {
+        uint4 v[U];
+#pragma unroll
+        for (int j = 0; j < U; j++) v[j] = ld_stream_u4(x8 + i + j * stride);
+#pragma unroll
+        for (int j = 0; j < U; j++) count8(v[j], true);
+    }
+    for (; warp_first + (i - first) < nv; i += stride) {
+        const bool ok = i < nv;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (ok) v = ld_stream_u4(x8 + i);
+        count8(v, ok);
+    }
+    const int64_t extra = head + (n - tail0);
+    if (warp_first < extra) {                                            // warp-uniform
+        const bool ok = first < extra;
+        float v = 0.f;
+        if (ok) v = ld_stream1_f(first < head ? x + first : x + tail0 + (first - head));
+        cnt.count(ok ? bin(v) : cnt.trash);
+    }
+}
+
 constexpr int kHistThreads = 1024;   // big CTAs: the flush of the private bins (bins global atomics per CTA) is what limits small-CTA
                                      // configurations (measured: 256 thr x 8/SM 59 % -> 1024 thr x 1/SM 82-86 % -> 1024 thr x 2/SM, two
                                      // loads in flight, 87 % of HBM peak: r02_kbench.txt)
-template <int VARIANT, class Bin, int U = kUnroll, int TPB = kHistThreads, int MINB = 1>
+template <int VARIANT, class Bin, int U = kUnroll, int TPB = kHistThreads, int MINB = 1, class T = float>
 __global__ void __launch_bounds__(TPB, MINB)
-histogram_kernel(const float *__restrict__ x, int64_t n, BinParams bp, int32_t *__restrict__ hist) {
+histogram_kernel(const T *__restrict__ x, int64_t n, BinParams bp, int32_t *__restrict__ hist) {
     extern __shared__ int sh[];
     const int bins = bp.bins;
     hist_zero<VARIANT>(sh, bins);
@@ -291,9 +361,9 @@ histogram_cluster_kernel(const float *__restrict__ x, int64_t n, BinParams bp, i
 }
 
 // hist_scale read from device memory (phase 2 without a host round trip); VARIANT 3 (global atomics) above kMaxSmemBins bins
-template <int VARIANT, int TPB = kHistThreads, int MINB = 2>
+template <int VARIANT, int TPB = kHistThreads, int MINB = 2, class T = float>
 __global__ void __launch_bounds__(TPB, MINB)
-histogram_dscale_kernel(const float *__restrict__ x, int64_t n, const float *__restrict__ hist_scale, int clip, int bins,
+histogram_dscale_kernel(const T *__restrict__ x, int64_t n, const float *__restrict__ hist_scale, int clip, int bins,
                         int32_t *__restrict__ hist) {
     extern __shared__ int sh[];
     hist_zero<VARIANT>(sh, bins);
@@ -531,6 +601,19 @@ static int launch_hist(const float *x, int64_t n, const BinParams &bin, int64_t 
     return (int)cudaGetLastError();
 }
 
+// fp16 / bf16: the default layout of launch_hist only (two 1024-thread CTAs per SM; global atomics beyond kMaxSmemBins bins)
+template <class Bin, class T>
+static int launch_hist_half(const T *x, int64_t n, const BinParams &bin, int64_t bins, int32_t *hist, cudaStream_t st) {
+    if (bins > kMaxSmemBins) {
+        histogram_kernel<3, Bin, kUnroll, kThreads, 1, T><<<grid_for(n, kThreads, 16, 8), kThreads, 0, st>>>(x, n, bin, hist);
+        return (int)cudaGetLastError();
+    }
+    const int grid = hist_grid(n, (int)bins);
+    histogram_kernel<0, Bin, 2, kHistThreads, 2, T><<<grid * 2 > sm_count() * 2 ? sm_count() * 2 : grid * 2, kHistThreads,
+                                                      (size_t)(bins + 1) * sizeof(int), st>>>(x, n, bin, hist);
+    return (int)cudaGetLastError();
+}
+
 // Two CTAs per SM when the ring, the prefix and the Op's shared memory allow it; each CTA should own >= 64 Ki elements before it pays
 // for its per-tensor set-up and publishes.  Rejects tables whose shared memory exceeds the device's opt-in limit.
 template <class Op>
@@ -568,24 +651,38 @@ int ppq_b200_minmax_init(float *mins, float *maxs, int64_t count, void *stream) 
     return (int)cudaGetLastError();
 }
 
-int ppq_b200_minmax_t(const float *x, int64_t n, float *minmax, void *stream) {
-    if (n <= 0 || !x || !minmax) return (int)cudaErrorInvalidValue;
-    const int grid = grid_for((n + 3) / 4, kThreads, kUnroll * 4, 8);
-    minmax_t_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(x, n, minmax);
-    return (int)cudaGetLastError();
+int ppq_b200_minmax_t_dt(const void *x, int dtype, int64_t n, float *minmax, void *stream) {
+    if (!valid_dtype(dtype) || n <= 0 || !x || !minmax) return (int)cudaErrorInvalidValue;
+    return with_elem_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        const int grid = grid_for((n + 16 / sizeof(T) - 1) / (16 / sizeof(T)), kThreads, kUnroll * 4, 8);
+        minmax_t_kernel<T><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const T *)x, n, minmax);
+        return (int)cudaGetLastError();
+    });
 }
 
-int ppq_b200_minmax_c(const float *x, int64_t n, int64_t epc, int C, float *mins, float *maxs, void *stream) {
-    if (n <= 0 || epc <= 0 || C <= 0 || !x || !mins || !maxs || n % epc != 0) return (int)cudaErrorInvalidValue;
+int ppq_b200_minmax_t(const float *x, int64_t n, float *minmax, void *stream) {
+    return ppq_b200_minmax_t_dt(x, PPQ_B200_F32, n, minmax, stream);
+}
+
+int ppq_b200_minmax_c_dt(const void *x, int dtype, int64_t n, int64_t epc, int C, float *mins, float *maxs, void *stream) {
+    if (!valid_dtype(dtype) || n <= 0 || epc <= 0 || C <= 0 || !x || !mins || !maxs || n % epc != 0) return (int)cudaErrorInvalidValue;
     const int64_t rows = n / epc;
     const int64_t chunks = (epc + kRowChunk - 1) / kRowChunk;
     if (chunks > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
     const int64_t items = rows * chunks;
     int64_t grid = (items + (kThreads / 32) - 1) / (kThreads / 32);
     if (grid > (int64_t)sm_count() * 8) grid = (int64_t)sm_count() * 8;
-    minmax_c_kernel<<<(int)grid, kThreads, 0, (cudaStream_t)stream>>>(x, rows, epc, C, chunks, FastDiv((uint32_t)chunks),
-                                                                          FastDiv((uint32_t)C), mins, maxs);
-    return (int)cudaGetLastError();
+    return with_elem_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        minmax_c_kernel<T><<<(int)grid, kThreads, 0, (cudaStream_t)stream>>>((const T *)x, rows, epc, C, chunks, FastDiv((uint32_t)chunks),
+                                                                             FastDiv((uint32_t)C), mins, maxs);
+        return (int)cudaGetLastError();
+    });
+}
+
+int ppq_b200_minmax_c(const float *x, int64_t n, int64_t epc, int C, float *mins, float *maxs, void *stream) {
+    return ppq_b200_minmax_c_dt(x, PPQ_B200_F32, n, epc, C, mins, maxs, stream);
 }
 
 int ppq_b200_histogram_t(const float *x, int64_t n, float hist_scale, int clip_outliers, int32_t *hist, int64_t bins, void *stream) {
@@ -593,24 +690,42 @@ int ppq_b200_histogram_t(const float *x, int64_t n, float hist_scale, int clip_o
     return launch_hist<SymBin>(x, n, BinParams{hist_scale, 0.f, (int)bins, clip_outliers}, bins, hist, (cudaStream_t)stream);
 }
 
+int ppq_b200_histogram_asym_t_dt(const void *x, int dtype, int64_t n, float vmin, float vmax, int clip_outliers, int32_t *hist, int64_t bins,
+                                 void *stream) {
+    if (!valid_dtype(dtype) || n <= 0 || !x || !hist || bins <= 0 || bins > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+    const BinParams bp{vmin, vmax, (int)bins, clip_outliers};
+    if (dtype == PPQ_B200_F32) return launch_hist<AsymBin>((const float *)x, n, bp, bins, hist, (cudaStream_t)stream);
+    return with_half_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        return launch_hist_half<AsymBin>((const T *)x, n, bp, bins, hist, (cudaStream_t)stream);
+    });
+}
+
 int ppq_b200_histogram_asym_t(const float *x, int64_t n, float vmin, float vmax, int clip_outliers, int32_t *hist, int64_t bins,
                               void *stream) {
-    if (n <= 0 || !x || !hist || bins <= 0 || bins > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-    return launch_hist<AsymBin>(x, n, BinParams{vmin, vmax, (int)bins, clip_outliers}, bins, hist, (cudaStream_t)stream);
+    return ppq_b200_histogram_asym_t_dt(x, PPQ_B200_F32, n, vmin, vmax, clip_outliers, hist, bins, stream);
+}
+
+int ppq_b200_histogram_t_dscale_dt(const void *x, int dtype, int64_t n, const float *hist_scale_dev, int clip_outliers, int32_t *hist,
+                                   int64_t bins, void *stream) {
+    if (!valid_dtype(dtype) || n <= 0 || !x || !hist || !hist_scale_dev || bins <= 0 || bins > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+    return with_elem_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        if (bins > kMaxSmemBins) {                 // the private bins do not fit: count with global atomics, as launch_hist does for Histogram_T
+            histogram_dscale_kernel<3, kThreads, 1, T><<<grid_for(n, kThreads, 16, 8), kThreads, 0, (cudaStream_t)stream>>>(
+                (const T *)x, n, hist_scale_dev, clip_outliers, (int)bins, hist);
+            return (int)cudaGetLastError();
+        }
+        const int grid = hist_grid(n, (int)bins) * 2 > sm_count() * 2 ? sm_count() * 2 : hist_grid(n, (int)bins) * 2;
+        histogram_dscale_kernel<0, kHistThreads, 2, T><<<grid, kHistThreads, (size_t)(bins + 1) * sizeof(int), (cudaStream_t)stream>>>(
+            (const T *)x, n, hist_scale_dev, clip_outliers, (int)bins, hist);
+        return (int)cudaGetLastError();
+    });
 }
 
 int ppq_b200_histogram_t_dscale(const float *x, int64_t n, const float *hist_scale_dev, int clip_outliers, int32_t *hist,
                                 int64_t bins, void *stream) {
-    if (n <= 0 || !x || !hist || !hist_scale_dev || bins <= 0 || bins > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-    if (bins > kMaxSmemBins) {                     // the private bins do not fit: count with global atomics, as launch_hist does for Histogram_T
-        histogram_dscale_kernel<3, kThreads, 1><<<grid_for(n, kThreads, 16, 8), kThreads, 0, (cudaStream_t)stream>>>(
-            x, n, hist_scale_dev, clip_outliers, (int)bins, hist);
-        return (int)cudaGetLastError();
-    }
-    const int grid = hist_grid(n, (int)bins) * 2 > sm_count() * 2 ? sm_count() * 2 : hist_grid(n, (int)bins) * 2;
-    histogram_dscale_kernel<0><<<grid, kHistThreads, (size_t)(bins + 1) * sizeof(int), (cudaStream_t)stream>>>(
-        x, n, hist_scale_dev, clip_outliers, (int)bins, hist);
-    return (int)cudaGetLastError();
+    return ppq_b200_histogram_t_dscale_dt(x, PPQ_B200_F32, n, hist_scale_dev, clip_outliers, hist, bins, stream);
 }
 
 int ppq_b200_histogram_c(const float *x, int64_t n, int64_t epc, int C, float hist_scale, int clip_outliers, int32_t *hist,

@@ -12,6 +12,7 @@
 // bandwidth-bound rather than issue-bound.  Variant 1 (ppq_b200_set_variant("linear_quant_t", 1)) is the
 // TMA-staged pipeline (cp.async.bulk global->shared ring with mbarriers, bulk store back) kept for comparison.
 #include "ops.cuh"
+#include "half.cuh"
 #include "../../include/ppq_b200.h"
 #include "variants.h"
 #include <string.h>
@@ -479,8 +480,152 @@ multi_tensor_kernel(const ppq_b200_lt_desc *__restrict__ descs, int count, typen
     }
 }
 
+// ---- half inputs (fp16 / bf16): 16-byte loads of 8 elements, the fp32 operator on the exact upcasts ----------------------------------------
+// A vector body starts at the input's first 16-byte boundary; the <= 7 elements before it and the <= 7 after the last whole vector are done
+// one by one.  Storage offsets from slicing usually leave the fresh output at a different alignment than the input: the body then stores
+// element by element (the loads stay 16 bytes wide).
+template <class Op, class OutT> struct EmitH {
+    static constexpr uintptr_t kVecAlign = sizeof(OutT) == 1 ? 4 : 16;     // int8: two 4-byte stores; half, int32: 16-byte stores
+    static __device__ __forceinline__ void one(const Op &op, float x, OutT *y) {
+        if constexpr (is_half_t<OutT>::value) *y = from_f<OutT>(op.apply(x));
+        else *y = Emit<Op, OutT>::one(op, x);
+    }
+    // elements [8 g, 8 g + 8) of y; `vec`: y is kVecAlign-aligned
+    static __device__ __forceinline__ void vec8(const Op &op, const float4 &a, const float4 &b, OutT *y, int64_t g, bool vec) {
+        if constexpr (is_half_t<OutT>::value) {
+            const float4 ra = op.apply4(a), rb = op.apply4(b);
+            if (vec) {
+                reinterpret_cast<uint4 *>(y)[g] = pack8<OutT>(ra, rb);
+            } else {
+                const float f[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
+#pragma unroll
+                for (int k = 0; k < 8; k++) y[8 * g + k] = from_f<OutT>(f[k]);
+            }
+        } else {
+            if (vec) {
+                Emit<Op, OutT>::vec(op, a, y, 2 * g);
+                Emit<Op, OutT>::vec(op, b, y, 2 * g + 1);
+            } else {
+                const int4 qa = op.quant4(a), qb = op.quant4(b);
+                const int q[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+#pragma unroll
+                for (int k = 0; k < 8; k++) y[8 * g + k] = (OutT)q[k];
+            }
+        }
+    }
+};
+
+template <class Op, class T, class OutT>
+__global__ void __launch_bounds__(kThreads)
+ew_half_tensor_kernel(const T *__restrict__ x, OutT *__restrict__ y, int64_t n,
+                      const float *__restrict__ scale, const float *__restrict__ offset, typename Op::Params p) {
+    const typename Op::Plan plan(p);
+    const Op op(plan, __ldg(scale), __ldg(offset));
+    const int64_t head = min(n, head_elems(x));
+    const int64_t nv = (n - head) >> 3, tail0 = head + (nv << 3);
+    const uint4 *x8 = reinterpret_cast<const uint4 *>(x + head);
+    OutT *yb = y + head;
+    const bool yvec = (reinterpret_cast<uintptr_t>(yb) & (EmitH<Op, OutT>::kVecAlign - 1)) == 0;
+    const int64_t tid = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * kThreads;
+    constexpr int64_t kSeg = 32 * kUnroll;                              // warp-contiguous segments, as in ew_tensor_kernel
+    const int64_t lane = threadIdx.x & 31, warp = tid >> 5, warps = stride >> 5;
+    const int64_t segs = (nv + kSeg - 1) / kSeg;
+    for (int64_t sg = warp; sg < segs; sg += warps) {
+        const int64_t base = sg * kSeg + lane;
+        uint4 v[kUnroll];
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) if (base + j * 32 < nv) v[j] = ld_stream_u4(x8 + base + j * 32);
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) {
+            if (base + j * 32 < nv) {
+                float4 a, b;
+                unpack8<T>(v[j], a, b);
+                EmitH<Op, OutT>::vec8(op, a, b, yb, base + j * 32, yvec);
+            }
+        }
+    }
+    if (tid < head) EmitH<Op, OutT>::one(op, ld_stream1_f(x + tid), y + tid);
+    else if (tid - head < n - tail0) EmitH<Op, OutT>::one(op, ld_stream1_f(x + tail0 + (tid - head)), y + tail0 + (tid - head));
+}
+
+// Per channel, any epc: the operator is built per 8-element vector (once when the vector lies in one channel row, which is always the case
+// when epc % 8 == 0 and the base is 16-byte aligned; otherwise rebuilt at each row end inside the vector).
+template <class Op, class T, class OutT>
+__global__ void __launch_bounds__(kThreads)
+ew_half_channel_kernel(const T *__restrict__ x, OutT *__restrict__ y, int64_t n, int64_t epc, int C, FastDiv div_epc, FastDiv div_C,
+                       const float *__restrict__ scale, const float *__restrict__ offset, typename Op::Params p) {
+    const typename Op::Plan plan(p);
+    const int64_t head = min(n, head_elems(x));
+    const int64_t nv = (n - head) >> 3, tail0 = head + (nv << 3);
+    const uint4 *x8 = reinterpret_cast<const uint4 *>(x + head);
+    OutT *yb = y + head;
+    const bool yvec = (reinterpret_cast<uintptr_t>(yb) & (EmitH<Op, OutT>::kVecAlign - 1)) == 0;
+    const int64_t tid = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * kThreads;
+    for (int64_t g0 = tid; g0 < nv; g0 += kUnroll * stride) {
+        uint4 v[kUnroll];
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) if (g0 + j * stride < nv) v[j] = ld_stream_u4(x8 + g0 + j * stride);
+#pragma unroll
+        for (int j = 0; j < kUnroll; j++) {
+            const int64_t g = g0 + j * stride;
+            if (g >= nv) continue;
+            const int64_t e0 = head + (g << 3);
+            const int64_t row = (int64_t)div_epc.quot((uint64_t)e0);
+            int64_t col = e0 - row * epc;
+            int c = (int)(row - (int64_t)div_C.quot((uint64_t)row) * C);
+            float4 a, b;
+            unpack8<T>(v[j], a, b);
+            if (col + 8 <= epc) {
+                const Op op(plan, __ldg(scale + c), __ldg(offset + c));
+                EmitH<Op, OutT>::vec8(op, a, b, yb, g, yvec);
+            } else {                                                    // the vector crosses a row end
+                const float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                Op op(plan, __ldg(scale + c), __ldg(offset + c));
+#pragma unroll
+                for (int k = 0; k < 8; k++) {
+                    EmitH<Op, OutT>::one(op, f[k], y + e0 + k);
+                    if (++col == epc) {
+                        col = 0; if (++c == C) c = 0;
+                        if (k < 7) op.rebind(__ldg(scale + c), __ldg(offset + c));
+                    }
+                }
+            }
+        }
+    }
+    int64_t e = -1;
+    if (tid < head) e = tid;
+    else if (tid - head < n - tail0) e = tail0 + (tid - head);
+    if (e >= 0) {
+        const int64_t row = (int64_t)div_epc.quot((uint64_t)e);
+        const int c = (int)(row - (int64_t)div_C.quot((uint64_t)row) * C);
+        const Op op(plan, __ldg(scale + c), __ldg(offset + c));
+        EmitH<Op, OutT>::one(op, ld_stream1_f(x + e), y + e);
+    }
+}
+
 // ---- host-side launch helpers --------------------------------------------------------------------------------------------
 static inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+template <class Op, class T, class OutT>
+static int launch_half_tensor(const void *x, void *y, int64_t n, const float *scale, const float *offset, typename Op::Params p,
+                              cudaStream_t st) {
+    if (n <= 0 || !x || !y || !scale || !offset) return (int)cudaErrorInvalidValue;
+    ew_half_tensor_kernel<Op, T, OutT><<<grid_for((n + 7) / 8, kThreads, kUnroll, 8), kThreads, 0, st>>>(
+        (const T *)x, (OutT *)y, n, scale, offset, p);
+    return (int)cudaGetLastError();
+}
+
+template <class Op, class T, class OutT>
+static int launch_half_channel(const void *x, void *y, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+                               typename Op::Params p, cudaStream_t st) {
+    if (n <= 0 || epc <= 0 || C <= 0 || !x || !y || !scale || !offset) return (int)cudaErrorInvalidValue;
+    if (epc > 0x7fffffffLL || n % epc != 0) return (int)cudaErrorInvalidValue;
+    ew_half_channel_kernel<Op, T, OutT><<<grid_for((n + 7) / 8, kThreads, kUnroll, 8), kThreads, 0, st>>>(
+        (const T *)x, (OutT *)y, n, epc, C, FastDiv((uint32_t)epc), FastDiv((uint32_t)C), scale, offset, p);
+    return (int)cudaGetLastError();
+}
 template <class OutT> static inline bool out_aligned(const void *p) {
     return (reinterpret_cast<uintptr_t>(p) & (4 * sizeof(OutT) - 1)) == 0;
 }
@@ -599,10 +744,19 @@ extern "C" {
     default: break;                                                 \
     }
 
-int ppq_b200_linear_quant_t(const float *x, float *y, int64_t n, const float *scale, const float *offset,
-                            int qmin, int qmax, int rounding, void *stream) {
+int ppq_b200_linear_quant_t_dt(const void *xv, int dtype, void *yv, int64_t n, const float *scale, const float *offset,
+                               int qmin, int qmax, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            PPQB_DISPATCH_MODE(rounding, return (launch_half_tensor<LinearOp<M_>, T, T>(xv, yv, n, scale, offset, {qmin, qmax, M_}, st)))
+            return launch_half_tensor<LinearOp<-1>, T, T>(xv, yv, n, scale, offset, {qmin, qmax, rounding}, st);
+        });
+    }
+    const float *x = (const float *)xv;
+    float *y = (float *)yv;
     if (rounding == RND_HALF_EVEN) {
         const int var = variant_of(kVarLinearT);
         if (var == 1 && n >= 4096 && aligned16(x) && aligned16(y))
@@ -620,21 +774,52 @@ int ppq_b200_linear_quant_t(const float *x, float *y, int64_t n, const float *sc
     return launch_tensor<LinearOp<-1>, float>(x, y, n, scale, offset, {qmin, qmax, rounding}, st);     // unknown ids: the reference's `default` branch
 }
 
-int ppq_b200_linear_quant_c(const float *x, float *y, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+int ppq_b200_linear_quant_t(const float *x, float *y, int64_t n, const float *scale, const float *offset,
                             int qmin, int qmax, int rounding, void *stream) {
+    return ppq_b200_linear_quant_t_dt(x, PPQ_B200_F32, y, n, scale, offset, qmin, qmax, rounding, stream);
+}
+
+int ppq_b200_linear_quant_c_dt(const void *xv, int dtype, void *yv, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+                               int qmin, int qmax, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            PPQB_DISPATCH_MODE(rounding, return (launch_half_channel<LinearOp<M_>, T, T>(xv, yv, n, epc, C, scale, offset, {qmin, qmax, M_}, st)))
+            return launch_half_channel<LinearOp<-1>, T, T>(xv, yv, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
+        });
+    }
+    const float *x = (const float *)xv;
+    float *y = (float *)yv;
     PPQB_DISPATCH_MODE(rounding, return (launch_channel<LinearOp<M_>, float>(x, y, n, epc, C, scale, offset, {qmin, qmax, M_}, st)))
     return launch_channel<LinearOp<-1>, float>(x, y, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
 }
 
+int ppq_b200_linear_quant_c(const float *x, float *y, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+                            int qmin, int qmax, int rounding, void *stream) {
+    return ppq_b200_linear_quant_c_dt(x, PPQ_B200_F32, y, n, epc, C, scale, offset, qmin, qmax, rounding, stream);
+}
+
 static int toint_bits_ok(int out_bits) { return out_bits == 8 || out_bits == 32; }
 
-int ppq_b200_linear_quant_t_toint(const float *x, void *q, int out_bits, int64_t n, const float *scale, const float *offset,
-                                  int qmin, int qmax, int rounding, void *stream) {
+int ppq_b200_linear_quant_t_toint_dt(const void *xv, int dtype, void *q, int out_bits, int64_t n, const float *scale, const float *offset,
+                                     int qmin, int qmax, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || qmin > qmax) return (int)cudaErrorInvalidValue;
     if (!toint_bits_ok(out_bits)) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            if (rounding == RND_HALF_EVEN) {
+                if (out_bits == 8) return launch_half_tensor<LinearOp<0>, T, int8_t>(xv, q, n, scale, offset, {qmin, qmax, 0}, st);
+                return launch_half_tensor<LinearOp<0>, T, int32_t>(xv, q, n, scale, offset, {qmin, qmax, 0}, st);
+            }
+            if (out_bits == 8) return launch_half_tensor<LinearOp<-1>, T, int8_t>(xv, q, n, scale, offset, {qmin, qmax, rounding}, st);
+            return launch_half_tensor<LinearOp<-1>, T, int32_t>(xv, q, n, scale, offset, {qmin, qmax, rounding}, st);
+        });
+    }
+    const float *x = (const float *)xv;
     if (rounding == RND_HALF_EVEN) {                                   // the policy every shipped quantizer but one selects: compile-time
         if (out_bits == 8) return launch_tensor<LinearOp<0>, int8_t>(x, (int8_t *)q, n, scale, offset, {qmin, qmax, 0}, st);
         return launch_tensor<LinearOp<0>, int32_t>(x, (int32_t *)q, n, scale, offset, {qmin, qmax, 0}, st);
@@ -643,17 +828,39 @@ int ppq_b200_linear_quant_t_toint(const float *x, void *q, int out_bits, int64_t
     return launch_tensor<LinearOp<-1>, int32_t>(x, (int32_t *)q, n, scale, offset, {qmin, qmax, rounding}, st);
 }
 
-int ppq_b200_linear_quant_c_toint(const float *x, void *q, int out_bits, int64_t n, int64_t epc, int C,
-                                  const float *scale, const float *offset, int qmin, int qmax, int rounding, void *stream) {
+int ppq_b200_linear_quant_t_toint(const float *x, void *q, int out_bits, int64_t n, const float *scale, const float *offset,
+                                  int qmin, int qmax, int rounding, void *stream) {
+    return ppq_b200_linear_quant_t_toint_dt(x, PPQ_B200_F32, q, out_bits, n, scale, offset, qmin, qmax, rounding, stream);
+}
+
+int ppq_b200_linear_quant_c_toint_dt(const void *xv, int dtype, void *q, int out_bits, int64_t n, int64_t epc, int C,
+                                     const float *scale, const float *offset, int qmin, int qmax, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (qmin > qmax) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || qmin > qmax) return (int)cudaErrorInvalidValue;
     if (!toint_bits_ok(out_bits)) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            if (rounding == RND_HALF_EVEN) {
+                if (out_bits == 8) return launch_half_channel<LinearOp<0>, T, int8_t>(xv, q, n, epc, C, scale, offset, {qmin, qmax, 0}, st);
+                return launch_half_channel<LinearOp<0>, T, int32_t>(xv, q, n, epc, C, scale, offset, {qmin, qmax, 0}, st);
+            }
+            if (out_bits == 8) return launch_half_channel<LinearOp<-1>, T, int8_t>(xv, q, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
+            return launch_half_channel<LinearOp<-1>, T, int32_t>(xv, q, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
+        });
+    }
+    const float *x = (const float *)xv;
     if (rounding == RND_HALF_EVEN) {
         if (out_bits == 8) return launch_channel<LinearOp<0>, int8_t>(x, (int8_t *)q, n, epc, C, scale, offset, {qmin, qmax, 0}, st);
         return launch_channel<LinearOp<0>, int32_t>(x, (int32_t *)q, n, epc, C, scale, offset, {qmin, qmax, 0}, st);
     }
     if (out_bits == 8) return launch_channel<LinearOp<-1>, int8_t>(x, (int8_t *)q, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
     return launch_channel<LinearOp<-1>, int32_t>(x, (int32_t *)q, n, epc, C, scale, offset, {qmin, qmax, rounding}, st);
+}
+
+int ppq_b200_linear_quant_c_toint(const float *x, void *q, int out_bits, int64_t n, int64_t epc, int C,
+                                  const float *scale, const float *offset, int qmin, int qmax, int rounding, void *stream) {
+    return ppq_b200_linear_quant_c_toint_dt(x, PPQ_B200_F32, q, out_bits, n, epc, C, scale, offset, qmin, qmax, rounding, stream);
 }
 
 int ppq_b200_multi_linear_quant_c(const ppq_b200_lc_desc *descs, int count, int64_t max_n, int qmin, int qmax, int rounding, void *stream) {
@@ -679,10 +886,22 @@ int ppq_b200_multi_linear_quant_t(const ppq_b200_lt_desc *descs, int count, int6
     return (int)cudaGetLastError();
 }
 
-int ppq_b200_float_quant_t(const float *x, float *y, int64_t n, const float *scale, const float *offset,
-                           int exponent, int mantissa, float clip_min, float clip_max, int rounding, void *stream) {
+int ppq_b200_float_quant_t_dt(const void *xv, int dtype, void *yv, int64_t n, const float *scale, const float *offset,
+                              int exponent, int mantissa, float clip_min, float clip_max, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (!valid_fp_format(exponent, mantissa)) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || !valid_fp_format(exponent, mantissa)) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            if (float_fast_path_ok(exponent, mantissa, clip_min, clip_max)) {
+                PPQB_DISPATCH_MODE(rounding, return (launch_half_tensor<FloatOp<M_, true>, T, T>(xv, yv, n, scale, offset, {exponent, mantissa, M_, clip_min, clip_max}, st)))
+            }
+            if (rounding == RND_HALF_EVEN) return launch_half_tensor<FloatOp<0>, T, T>(xv, yv, n, scale, offset, {exponent, mantissa, 0, clip_min, clip_max}, st);
+            return launch_half_tensor<FloatOp<-1>, T, T>(xv, yv, n, scale, offset, {exponent, mantissa, rounding, clip_min, clip_max}, st);
+        });
+    }
+    const float *x = (const float *)xv;
+    float *y = (float *)yv;
     if (float_fast_path_ok(exponent, mantissa, clip_min, clip_max)) {
         PPQB_DISPATCH_MODE(rounding, return (launch_tensor<FloatOp<M_, true>, float>(x, y, n, scale, offset, {exponent, mantissa, M_, clip_min, clip_max}, st)))
     }
@@ -690,15 +909,37 @@ int ppq_b200_float_quant_t(const float *x, float *y, int64_t n, const float *sca
     return launch_tensor<FloatOp<-1>, float>(x, y, n, scale, offset, {exponent, mantissa, rounding, clip_min, clip_max}, st);
 }
 
-int ppq_b200_float_quant_c(const float *x, float *y, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+int ppq_b200_float_quant_t(const float *x, float *y, int64_t n, const float *scale, const float *offset,
                            int exponent, int mantissa, float clip_min, float clip_max, int rounding, void *stream) {
+    return ppq_b200_float_quant_t_dt(x, PPQ_B200_F32, y, n, scale, offset, exponent, mantissa, clip_min, clip_max, rounding, stream);
+}
+
+int ppq_b200_float_quant_c_dt(const void *xv, int dtype, void *yv, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+                              int exponent, int mantissa, float clip_min, float clip_max, int rounding, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (!valid_fp_format(exponent, mantissa)) return (int)cudaErrorInvalidValue;
+    if (!valid_dtype(dtype) || !valid_fp_format(exponent, mantissa)) return (int)cudaErrorInvalidValue;
+    if (dtype != PPQ_B200_F32) {
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            if (float_fast_path_ok(exponent, mantissa, clip_min, clip_max)) {
+                PPQB_DISPATCH_MODE(rounding, return (launch_half_channel<FloatOp<M_, true>, T, T>(xv, yv, n, epc, C, scale, offset, {exponent, mantissa, M_, clip_min, clip_max}, st)))
+            }
+            if (rounding == RND_HALF_EVEN) return launch_half_channel<FloatOp<0>, T, T>(xv, yv, n, epc, C, scale, offset, {exponent, mantissa, 0, clip_min, clip_max}, st);
+            return launch_half_channel<FloatOp<-1>, T, T>(xv, yv, n, epc, C, scale, offset, {exponent, mantissa, rounding, clip_min, clip_max}, st);
+        });
+    }
+    const float *x = (const float *)xv;
+    float *y = (float *)yv;
     if (float_fast_path_ok(exponent, mantissa, clip_min, clip_max)) {
         PPQB_DISPATCH_MODE(rounding, return (launch_channel<FloatOp<M_, true>, float>(x, y, n, epc, C, scale, offset, {exponent, mantissa, M_, clip_min, clip_max}, st)))
     }
     if (rounding == RND_HALF_EVEN) return launch_channel<FloatOp<0>, float>(x, y, n, epc, C, scale, offset, {exponent, mantissa, 0, clip_min, clip_max}, st);
     return launch_channel<FloatOp<-1>, float>(x, y, n, epc, C, scale, offset, {exponent, mantissa, rounding, clip_min, clip_max}, st);
+}
+
+int ppq_b200_float_quant_c(const float *x, float *y, int64_t n, int64_t epc, int C, const float *scale, const float *offset,
+                           int exponent, int mantissa, float clip_min, float clip_max, int rounding, void *stream) {
+    return ppq_b200_float_quant_c_dt(x, PPQ_B200_F32, y, n, epc, C, scale, offset, exponent, mantissa, clip_min, clip_max, rounding, stream);
 }
 
 }  // extern "C"

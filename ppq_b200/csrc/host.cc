@@ -25,7 +25,7 @@ static int key_of(const char *name) {
 
 extern "C" {
 
-int ppq_b200_abi_version(void) { return 1; }
+int ppq_b200_abi_version(void) { return 2; }
 
 const char *ppq_b200_error_string(int status) {
     if (status == 0) return "success";
@@ -33,7 +33,7 @@ const char *ppq_b200_error_string(int status) {
 }
 
 const char *ppq_b200_build_info(void) {
-    return "libppq_b200 abi 1; sm_90a; host compiler gcc " __VERSION__ "; built " __DATE__;
+    return "libppq_b200 abi 2; sm_90a; host compiler gcc " __VERSION__ "; built " __DATE__;
 }
 
 int ppq_b200_set_variant(const char *kernel, int variant) {

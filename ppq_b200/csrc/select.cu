@@ -25,6 +25,7 @@
 // No allocation -- the caller provides the workspace.  The result is the identical element, bit for bit, except that a selected zero is
 // reported with the sign its key order gives (-0.0 < +0.0), equal as a float to whichever zero the reference's sort left at that index.
 #include "common.cuh"
+#include "half.cuh"
 #include "variants.h"
 #include "../../include/ppq_b200.h"
 
@@ -161,12 +162,13 @@ __device__ __forceinline__ void cta_select_two(const uint32_t (&key)[PER], long 
 }
 
 // The sample itself is drawn by a grid of small CTAs (16 K scattered 32-byte sectors are ~25 us for one SM's miss queue and ~2 us for 64 SMs).
+template <class T>
 __global__ void __launch_bounds__(256)
-select_sample_kernel(const float *__restrict__ x, int64_t n, uint32_t *__restrict__ keys) {
+select_sample_kernel(const T *__restrict__ x, int64_t n, uint32_t *__restrict__ keys) {
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     const int64_t stride = n / kSampleKeys;
     const int64_t off = (int64_t)((uint64_t)(i * 0x9E3779B1u) % (uint64_t)stride);
-    keys[i] = order_key(__ldg(x + (int64_t)i * stride + off));
+    keys[i] = order_key(to_f(__ldg(x + (int64_t)i * stride + off)));
 }
 
 // one CTA per tensor.  q_mode: ranks = {rn(n q), rn(n (1 - q))};  otherwise explicit ranks (isotone).  sample_keys != nullptr (single tensor,
@@ -307,6 +309,39 @@ __device__ __forceinline__ void stream_range(const float *__restrict__ x, int64_
     }
 }
 
+// fp16 / bf16: 16-byte loads of 8 elements, visited as two float4 of their exact upcasts; the <= 7 + 7 elements before the first 16-byte
+// boundary and after the last whole vector go one per thread to the first threads of the group.
+template <int U, bool SEGMENTS, class T, class F4, class F1, std::enable_if_t<is_half_t<T>::value, int> = 0>
+__device__ __forceinline__ void stream_range(const T *__restrict__ x, int64_t a, int64_t b, int64_t first, int64_t stride, F4 &&visit4, F1 &&visit1) {
+    const T *p = x + a;
+    const int64_t n = b - a;
+    const int64_t head = min(n, head_elems(p));
+    const int64_t nv = (n - head) >> 3, tail0 = head + (nv << 3);
+    const uint4 *x8 = reinterpret_cast<const uint4 *>(p + head);
+    auto visit8 = [&](const uint4 &r) { float4 lo, hi; unpack8<T>(r, lo, hi); visit4(lo); visit4(hi); };
+    if (!SEGMENTS) {
+        for (int64_t i = first; i < nv; i += U * stride) {
+            uint4 v[U];
+#pragma unroll
+            for (int j = 0; j < U; j++) if (i + j * stride < nv) v[j] = ld_stream_u4(x8 + i + j * stride);
+#pragma unroll
+            for (int j = 0; j < U; j++) if (i + j * stride < nv) visit8(v[j]);
+        }
+    } else {
+        const int64_t lane = first & 31, warps = stride >> 5;
+        for (int64_t sg = first >> 5; sg * (32 * U) < nv; sg += warps) {
+            const int64_t base = sg * (32 * U) + lane;
+            uint4 v[U];
+#pragma unroll
+            for (int j = 0; j < U; j++) if (base + j * 32 < nv) v[j] = ld_stream_u4(x8 + base + j * 32);
+#pragma unroll
+            for (int j = 0; j < U; j++) if (base + j * 32 < nv) visit8(v[j]);
+        }
+    }
+    if (first < head) visit1(ld_stream1_f(p + first));
+    else if (first - head < n - tail0) visit1(ld_stream1_f(p + tail0 + (first - head)));
+}
+
 // Does this tensor need a streaming pass at LEVEL?  (uniform over the grid: it only reads what the previous scan wrote)
 template <int LEVEL>
 __device__ __forceinline__ bool level_needed(const SelectState *st) {
@@ -319,8 +354,8 @@ __device__ __forceinline__ bool level_needed(const SelectState *st) {
 
 // One pass over the part [a, b) of a tensor for the CTA (`first`, `stride` in threads of the cooperating group).  Returns false when the
 // tensor needs nothing at this level (uniform over the grid).
-template <int LEVEL, int TPB, int U = 4, bool SEG = (LEVEL != 0)>
-__device__ __forceinline__ bool select_pass(const float *__restrict__ x, int64_t a, int64_t b, int64_t first, int64_t stride,
+template <int LEVEL, int TPB, int U = 4, bool SEG = (LEVEL != 0), class T = float>
+__device__ __forceinline__ bool select_pass(const T *__restrict__ x, int64_t a, int64_t b, int64_t first, int64_t stride,
                                             SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap, int (*sh)[kDigits], unsigned int *sh_cnt) {
     constexpr int shift = level_shift(LEVEL);
     constexpr uint32_t dmask = level_dmask(LEVEL), pmask = level_pmask(LEVEL);
@@ -394,8 +429,8 @@ template <int TPB> __device__ __forceinline__ void finish_tensor_pass(SelectStat
 // beyond the thresholds remembered from the previous call of this slot (the previous batch of the same activation: the tail moves little
 // from batch to batch) is compacted -- except copies of the previously selected key, which are only counted.  When the candidates turn out
 // to contain the requested order statistics (select_scan<0>), the finish selects among them and the tensor has been read ONCE.
-template <int TPB>
-__device__ __forceinline__ void select_pass0_spec(const float *__restrict__ x, int64_t a, int64_t b, int64_t first, int64_t stride,
+template <int TPB, class T = float>
+__device__ __forceinline__ void select_pass0_spec(const T *__restrict__ x, int64_t a, int64_t b, int64_t first, int64_t stride,
                                                   SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap, int (*sh)[kDigits], unsigned int *sh_cnt) {
     constexpr int kHalf = kStage / 2;                                     // sh[1] holds both staging lists: hi candidates, then lo candidates
     const uint32_t g_hi = st->g[0], k_hi = st->k[0], g_lo = st->g[1], k_lo = st->k[1];
@@ -435,12 +470,13 @@ __device__ __forceinline__ void select_pass0_spec(const float *__restrict__ x, i
     }
 }
 
+template <class T>
 __global__ void __launch_bounds__(kSelThreads, 1)
-select_pass0_spec_kernel(const float *__restrict__ x, int64_t n, SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap) {
+select_pass0_spec_kernel(const T *__restrict__ x, int64_t n, SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap) {
     __shared__ int sh[2][kDigits];
     __shared__ unsigned int sh_cnt[2];
     __shared__ bool is_last;
-    select_pass0_spec<kSelThreads>(x, 0, n, (int64_t)blockIdx.x * kSelThreads + threadIdx.x, (int64_t)gridDim.x * kSelThreads, st, bufs, cap, sh, sh_cnt);
+    select_pass0_spec<kSelThreads, T>(x, 0, n, (int64_t)blockIdx.x * kSelThreads + threadIdx.x, (int64_t)gridDim.x * kSelThreads, st, bufs, cap, sh, sh_cnt);
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) is_last = (atomicAdd(&st->done, 1u) == gridDim.x - 1);
@@ -488,13 +524,13 @@ multi_select_pass0_spec_kernel(const ppq_b200_tensor_desc *__restrict__ descs, i
 }
 
 // ---- single tensor: the whole grid interleaves over the tensor, the last CTA to finish resolves the pass ------------------------------
-template <int LEVEL, int TPB, int U = 4, bool SEG = (LEVEL != 0), int CTAS = (LEVEL == 0 ? 2 : 6)>
+template <int LEVEL, int TPB, int U = 4, bool SEG = (LEVEL != 0), int CTAS = (LEVEL == 0 ? 2 : 6), class T = float>
 __global__ void __launch_bounds__(TPB, CTAS)
-select_pass_kernel(const float *__restrict__ x, int64_t n, SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap) {
+select_pass_kernel(const T *__restrict__ x, int64_t n, SelectState *__restrict__ st, uint32_t *__restrict__ bufs, int64_t cap) {
     __shared__ int sh[2][kDigits];
     __shared__ unsigned int sh_cnt[2];
     __shared__ bool is_last;
-    if (!select_pass<LEVEL, TPB, U, SEG>(x, 0, n, (int64_t)blockIdx.x * TPB + threadIdx.x, (int64_t)gridDim.x * TPB, st, bufs, cap, sh, sh_cnt)) return;
+    if (!select_pass<LEVEL, TPB, U, SEG, T>(x, 0, n, (int64_t)blockIdx.x * TPB + threadIdx.x, (int64_t)gridDim.x * TPB, st, bufs, cap, sh, sh_cnt)) return;
     // every CTA's atomics are ordered before its ticket
     __threadfence();
     __syncthreads();
@@ -647,7 +683,11 @@ static inline int grid_filter(int64_t n) {
     return (int)(g < 1 ? 1 : g);
 }
 
-static int select_two(const float *x, int64_t n, int q_mode, float q, long long r0, long long r1, float *out, void *workspace, cudaStream_t s,
+// passes 1-2 at six CTAs per SM (40 registers) for fp32; the half unpacking needs a few more registers (five CTAs per SM, no spill)
+template <class T> constexpr int kFilterCtas = std::is_same<T, float>::value ? 6 : 5;
+
+template <class T>
+static int select_two(const T *x, int64_t n, int q_mode, float q, long long r0, long long r1, float *out, void *workspace, cudaStream_t s,
                       uint32_t *guess = nullptr) {
     SelectState *st = (SelectState *)workspace;
     uint32_t *bufs = (uint32_t *)(st + 1);
@@ -660,11 +700,13 @@ static int select_two(const float *x, int64_t n, int q_mode, float q, long long 
         sample = sample_rank_ok(sample_rank_from_end(need_hi, n), n, cap) || sample_rank_ok(sample_rank_from_end(need_lo, n), n, cap);
     }
     uint32_t *sample_keys = bufs + 2 * cap;
-    if (sample) select_sample_kernel<<<kSampleKeys / 256, 256, 0, s>>>(x, n, sample_keys);
+    if (sample) select_sample_kernel<T><<<kSampleKeys / 256, 256, 0, s>>>(x, n, sample_keys);
     select_init_kernel<<<1, 1024, 0, s>>>(st, nullptr, n, q, q_mode, r0, r1, guess, sample ? sample_keys : nullptr, cap);
     if (guess || sample) {
         const int g0 = grid_pass0(n);
-        select_pass0_spec_kernel<<<g0 > sm_count() ? sm_count() : g0, kSelThreads, 0, s>>>(x, n, st, bufs, cap);
+        select_pass0_spec_kernel<T><<<g0 > sm_count() ? sm_count() : g0, kSelThreads, 0, s>>>(x, n, st, bufs, cap);
+    } else if constexpr (!std::is_same<T, float>::value) {              // the A/B knobs below are fp32 only
+        select_pass_kernel<0, kSelThreads, 2, false, 2, T><<<grid_pass0(n), kSelThreads, 0, s>>>(x, n, st, bufs, cap);   // 2 x 16 B in flight: 32 registers, no spill
     } else {
         switch (variant_of(kVarSelect) & 7) {                              // A/B knobs of pass 0 (variants.h)
         case 1: select_pass_kernel<0, kSelThreads, 2><<<grid_pass0(n), kSelThreads, 0, s>>>(x, n, st, bufs, cap); break;
@@ -674,16 +716,20 @@ static int select_two(const float *x, int64_t n, int q_mode, float q, long long 
         default: select_pass_kernel<0, kSelThreads><<<grid_pass0(n), kSelThreads, 0, s>>>(x, n, st, bufs, cap);
         }
     }
-    switch ((variant_of(kVarSelect) >> 3) & 7) {                                 // ... and of pass 1
-    case 1: select_pass_kernel<1, kFilterThreads, 2><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
-    case 2: select_pass_kernel<1, 512, 4, true, 3><<<grid_filter(n) / 2, 512, 0, s>>>(x, n, st, bufs, cap); break;
-    case 3: select_pass_kernel<1, 1024, 2, true, 2><<<grid_pass0(n), 1024, 0, s>>>(x, n, st, bufs, cap); break;
-    case 4: select_pass_kernel<1, kFilterThreads, 4, false><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
-    default: select_pass_kernel<1, kFilterThreads><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap);
+    if constexpr (!std::is_same<T, float>::value) {
+        select_pass_kernel<1, kFilterThreads, 4, true, kFilterCtas<T>, T><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap);
+    } else {
+        switch ((variant_of(kVarSelect) >> 3) & 7) {                             // ... and of pass 1
+        case 1: select_pass_kernel<1, kFilterThreads, 2><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
+        case 2: select_pass_kernel<1, 512, 4, true, 3><<<grid_filter(n) / 2, 512, 0, s>>>(x, n, st, bufs, cap); break;
+        case 3: select_pass_kernel<1, 1024, 2, true, 2><<<grid_pass0(n), 1024, 0, s>>>(x, n, st, bufs, cap); break;
+        case 4: select_pass_kernel<1, kFilterThreads, 4, false><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
+        default: select_pass_kernel<1, kFilterThreads><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap);
+        }
     }
     // pass 2 is rarely needed (a bucket too big to compact that holds several distinct values): two CTAs per SM keep its usual early exit cheap
     const int g2 = grid_filter(n) > 2 * sm_count() ? 2 * sm_count() : grid_filter(n);
-    select_pass_kernel<2, kFilterThreads><<<g2, kFilterThreads, 0, s>>>(x, n, st, bufs, cap);
+    select_pass_kernel<2, kFilterThreads, 4, true, kFilterCtas<T>, T><<<g2, kFilterThreads, 0, s>>>(x, n, st, bufs, cap);
     select_finish_kernel<<<2, kSelThreads, 0, s>>>(st, bufs, cap, nullptr, out, 0, guess);
     return (int)cudaGetLastError();
 }
@@ -712,14 +758,20 @@ int64_t ppq_b200_multi_quantile_workspace_bytes(int count, int64_t cap) {
     return (int64_t)count * ((int64_t)sizeof(SelectState) + 2 * cap * (int64_t)sizeof(uint32_t));
 }
 
+int ppq_b200_quantile_t_dt(const void *x, int dtype, int64_t n, float q, float *out2, void *workspace, uint32_t *guess, void *stream) {
+    if (!valid_dtype(dtype) || n <= 0 || !x || !out2 || !workspace) return (int)cudaErrorInvalidValue;
+    return with_elem_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        return select_two((const T *)x, n, 1, q, 0, 0, out2, workspace, (cudaStream_t)stream, guess);
+    });
+}
+
 int ppq_b200_quantile_t(const float *x, int64_t n, float q, float *out2, void *workspace, void *stream) {
-    if (n <= 0 || !x || !out2 || !workspace) return (int)cudaErrorInvalidValue;
-    return select_two(x, n, 1, q, 0, 0, out2, workspace, (cudaStream_t)stream);
+    return ppq_b200_quantile_t_dt(x, PPQ_B200_F32, n, q, out2, workspace, nullptr, stream);
 }
 
 int ppq_b200_quantile_t_guess(const float *x, int64_t n, float q, float *out2, void *workspace, uint32_t *guess, void *stream) {
-    if (n <= 0 || !x || !out2 || !workspace) return (int)cudaErrorInvalidValue;
-    return select_two(x, n, 1, q, 0, 0, out2, workspace, (cudaStream_t)stream, guess);
+    return ppq_b200_quantile_t_dt(x, PPQ_B200_F32, n, q, out2, workspace, guess, stream);
 }
 
 int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float q, float *out, int64_t out_stride,

@@ -32,6 +32,17 @@ void CheckTensor(const Tensor &t, c10::ScalarType type, const char *name) {     
     if (t.numel() == 0) throw KernelFailure(std::string("Kernel Failure, Tensor is empty: ") + name);
     if (!t.is_cuda()) throw KernelFailure(std::string("Kernel Failure, Tensor is not on a CUDA device: ") + name);
 }
+// A value tensor of fp32, fp16 or bf16 (half_only: fp16 or bf16); returns its element-type code in the C ABI.
+int CheckValue(const Tensor &t, bool half_only) {
+    const auto st = at::typeMetaToScalarType(t.dtype());
+    const int code = st == at::kHalf ? PPQ_B200_F16 : st == at::kBFloat16 ? PPQ_B200_BF16 : (st == at::kFloat && !half_only) ? PPQ_B200_F32 : -1;
+    if (code < 0)
+        throw KernelFailure(std::string("Kernel Failure, Invalid dtype of Input tensor: ") +
+                            (half_only ? "Value(Expect to be FP16 or BF16)" : "Value(Expect to be FP32, FP16 or BF16)"));
+    if (t.numel() == 0) throw KernelFailure("Kernel Failure, Tensor is empty: Value");
+    if (!t.is_cuda()) throw KernelFailure("Kernel Failure, Tensor is not on a CUDA device: Value");
+    return code;
+}
 void CheckStatus(int status, const char *what) {
     if (status != 0) throw KernelFailure(std::string("Kernel Failure, ") + what + ": " + ppq_b200_error_string(status));
 }
@@ -100,7 +111,7 @@ Tensor QuantizeTensor_LC(const Tensor &value, const Tensor &scale, const Tensor 
 // device twin of PPQLinearQuant_toInt (ppq/quantization/qfunction/linear.py:218-238); channel_axis < -100 means per-tensor
 Tensor QuantizeTensor_toInt(const Tensor &value, const Tensor &scale, const Tensor &offset, const int clip_min, const int clip_max,
                             const int channel_axis, const int rounding, const int out_bits) {
-    CheckTensor(value, at::kFloat, "Value(Expect to be FP32)");
+    const int dt = CheckValue(value, false);
     CheckTensor(scale, at::kFloat, "Scale(Expect to be FP32)");
     CheckTensor(offset, at::kFloat, "Offset(Expect to be FP32)");
     CheckSize(value);
@@ -110,13 +121,13 @@ Tensor QuantizeTensor_toInt(const Tensor &value, const Tensor &scale, const Tens
     const auto dtype = out_bits == 32 ? at::kInt : ((clip_min >= 0 && clip_max > 127) ? at::kByte : at::kChar);
     Tensor out = at::empty(v.sizes(), v.options().dtype(dtype));
     if (channel_axis < -100) {
-        CheckStatus(ppq_b200_linear_quant_t_toint(F(v), out.data_ptr(), out_bits, v.numel(), F(s), F(o), clip_min, clip_max, rounding,
-                                                  Stream()), "QuantizeTensor_toInt");
+        CheckStatus(ppq_b200_linear_quant_t_toint_dt(v.data_ptr(), dt, out.data_ptr(), out_bits, v.numel(), F(s), F(o), clip_min, clip_max,
+                                                     rounding, Stream()), "QuantizeTensor_toInt");
     } else {
         const Geometry g = ChannelGeometry(v, channel_axis);
         CheckChannelParams(s, o, g.C);
-        CheckStatus(ppq_b200_linear_quant_c_toint(F(v), out.data_ptr(), out_bits, v.numel(), g.epc, g.C, F(s), F(o), clip_min,
-                                                  clip_max, rounding, Stream()), "QuantizeTensor_toInt");
+        CheckStatus(ppq_b200_linear_quant_c_toint_dt(v.data_ptr(), dt, out.data_ptr(), out_bits, v.numel(), g.epc, g.C, F(s), F(o), clip_min,
+                                                     clip_max, rounding, Stream()), "QuantizeTensor_toInt");
     }
     return out;
 }
@@ -149,6 +160,80 @@ Tensor QuantizeTensor_FC(const Tensor &value, const Tensor &scale, const Tensor 
     CheckStatus(ppq_b200_float_quant_c(F(v), out.data_ptr<float>(), v.numel(), g.epc, g.C, F(s), F(o), exponent, mantissa, clip_min,
                                        clip_max, rounding, Stream()), "QuantizeTensor_FC");
     return out;
+}
+
+// ---------------------------------------------------------------- fp16 / bf16 siblings of the fake-quant names
+// Same positional signatures; the value is fp16 or bf16 and so is the output (the fp32 result on the exact upcast, rounded once to nearest
+// even).  Scale and offset stay fp32.  The reference names above keep their fp32-only checks.
+Tensor QuantizeTensor_LT_Half(const Tensor &value, const Tensor &scale, const Tensor &offset, const int clip_min, const int clip_max,
+                              const int rounding) {
+    const int dt = CheckValue(value, true);
+    CheckTensor(scale, at::kFloat, "Scale(Expect to be FP32)");
+    CheckTensor(offset, at::kFloat, "Offset(Expect to be FP32)");
+    CheckSize(value);
+    const c10::cuda::CUDAGuard guard(value.device());
+    auto v = DenseFormat(value);
+    Tensor out = at::empty_like(v);
+    CheckStatus(ppq_b200_linear_quant_t_dt(v.data_ptr(), dt, out.data_ptr(), v.numel(), F(scale), F(offset), clip_min, clip_max, rounding,
+                                           Stream()), "QuantizeTensor_LT_Half");
+    return out;
+}
+
+Tensor QuantizeTensor_LC_Half(const Tensor &value, const Tensor &scale, const Tensor &offset, const int clip_min, const int clip_max,
+                              const int channel_axis, const int rounding) {
+    const int dt = CheckValue(value, true);
+    CheckTensor(scale, at::kFloat, "Scale(Expect to be FP32)");
+    CheckTensor(offset, at::kFloat, "Offset(Expect to be FP32)");
+    CheckSize(value);
+    const c10::cuda::CUDAGuard guard(value.device());
+    auto v = value.contiguous();
+    auto s = scale.contiguous(), o = offset.contiguous();
+    const Geometry g = ChannelGeometry(v, channel_axis);
+    CheckChannelParams(s, o, g.C);
+    Tensor out = at::empty_like(v);
+    CheckStatus(ppq_b200_linear_quant_c_dt(v.data_ptr(), dt, out.data_ptr(), v.numel(), g.epc, g.C, F(s), F(o), clip_min, clip_max, rounding,
+                                           Stream()), "QuantizeTensor_LC_Half");
+    return out;
+}
+
+Tensor QuantizeTensor_FT_Half(const Tensor &value, const Tensor &scale, const Tensor &offset, const int exponent, const int mantissa,
+                              const float clip_min, const float clip_max, const int rounding) {
+    const int dt = CheckValue(value, true);
+    CheckTensor(scale, at::kFloat, "Scale(Expect to be FP32)");
+    CheckTensor(offset, at::kFloat, "Offset(Expect to be FP32)");
+    CheckSize(value);
+    const c10::cuda::CUDAGuard guard(value.device());
+    auto v = DenseFormat(value);
+    Tensor out = at::empty_like(v);
+    CheckStatus(ppq_b200_float_quant_t_dt(v.data_ptr(), dt, out.data_ptr(), v.numel(), F(scale), F(offset), exponent, mantissa, clip_min,
+                                          clip_max, rounding, Stream()), "QuantizeTensor_FT_Half");
+    return out;
+}
+
+Tensor QuantizeTensor_FC_Half(const Tensor &value, const Tensor &scale, const Tensor &offset, const int exponent, const int mantissa,
+                              const float clip_min, const float clip_max, const int channel_axis, const int rounding) {
+    const int dt = CheckValue(value, true);
+    CheckTensor(scale, at::kFloat, "Scale(Expect to be FP32)");
+    CheckTensor(offset, at::kFloat, "Offset(Expect to be FP32)");
+    CheckSize(value);
+    const c10::cuda::CUDAGuard guard(value.device());
+    auto v = value.contiguous();
+    auto s = scale.contiguous(), o = offset.contiguous();
+    const Geometry g = ChannelGeometry(v, channel_axis);
+    CheckChannelParams(s, o, g.C);
+    Tensor out = at::empty_like(v);
+    CheckStatus(ppq_b200_float_quant_c_dt(v.data_ptr(), dt, out.data_ptr(), v.numel(), g.epc, g.C, F(s), F(o), exponent, mantissa, clip_min,
+                                          clip_max, rounding, Stream()), "QuantizeTensor_FC_Half");
+    return out;
+}
+
+void Histogram_Asymmetric_T_Half(const float min, const float max, const Tensor &value, const bool clip_outliers, Tensor &hist) {
+    const int dt = CheckValue(value, true);
+    CheckTensor(hist, at::kInt, "Histogram(Expect to be INT32)");
+    const c10::cuda::CUDAGuard guard(value.device());
+    auto v = Dense(value);
+    CheckStatus(ppq_b200_histogram_asym_t_dt(v.data_ptr(), dt, v.numel(), min, max, clip_outliers, hist.data_ptr<int>(), hist.numel(), Stream()),
+                "Histogram_Asymmetric_T_Half");
 }
 
 // ---------------------------------------------------------------- histograms (sort.h:5-23)
@@ -194,30 +279,30 @@ void MinMax_Init(Tensor &mins, Tensor &maxs) {
 }
 // minmax: float[2] = {min, max}, accumulated
 void MinMax_T(const Tensor &value, Tensor &minmax) {
-    CheckTensor(value, at::kFloat, "Value(Expect to be FP32)");
+    const int dt = CheckValue(value, false);
     CheckTensor(minmax, at::kFloat, "MinMax(Expect to be FP32)");
     if (minmax.numel() != 2) throw KernelFailure("Kernel Failure, MinMax buffer must hold 2 floats.");
     const c10::cuda::CUDAGuard guard(value.device());
     auto v = Dense(value);
-    CheckStatus(ppq_b200_minmax_t(F(v), v.numel(), minmax.data_ptr<float>(), Stream()), "MinMax_T");
+    CheckStatus(ppq_b200_minmax_t_dt(v.data_ptr(), dt, v.numel(), minmax.data_ptr<float>(), Stream()), "MinMax_T");
 }
 void MinMax_C(const Tensor &value, const int channel_axis, Tensor &mins, Tensor &maxs) {
-    CheckTensor(value, at::kFloat, "Value(Expect to be FP32)");
+    const int dt = CheckValue(value, false);
     CheckTensor(mins, at::kFloat, "Min(Expect to be FP32)");
     CheckTensor(maxs, at::kFloat, "Max(Expect to be FP32)");
     const c10::cuda::CUDAGuard guard(value.device());
     auto v = value.contiguous();
     const Geometry g = ChannelGeometry(v, channel_axis);
     if (mins.numel() != g.C || maxs.numel() != g.C) throw KernelFailure("Kernel Failure, min / max must hold one value per channel.");
-    CheckStatus(ppq_b200_minmax_c(F(v), v.numel(), g.epc, g.C, mins.data_ptr<float>(), maxs.data_ptr<float>(), Stream()), "MinMax_C");
+    CheckStatus(ppq_b200_minmax_c_dt(v.data_ptr(), dt, v.numel(), g.epc, g.C, mins.data_ptr<float>(), maxs.data_ptr<float>(), Stream()), "MinMax_C");
 }
 void Histogram_T_DeviceScale(const Tensor &value, const Tensor &hist_scale, const bool clip_outliers, Tensor &hist) {
-    CheckTensor(value, at::kFloat, "Value(Expect to be FP32)");
+    const int dt = CheckValue(value, false);
     CheckTensor(hist_scale, at::kFloat, "HistScale(Expect to be FP32)");
     CheckTensor(hist, at::kInt, "Histogram(Expect to be INT32)");
     const c10::cuda::CUDAGuard guard(value.device());
     auto v = Dense(value);
-    CheckStatus(ppq_b200_histogram_t_dscale(F(v), v.numel(), F(hist_scale), clip_outliers, hist.data_ptr<int>(), hist.numel(), Stream()),
+    CheckStatus(ppq_b200_histogram_t_dscale_dt(v.data_ptr(), dt, v.numel(), F(hist_scale), clip_outliers, hist.data_ptr<int>(), hist.numel(), Stream()),
                 "Histogram_T_DeviceScale");
 }
 // descs: int64 tensor [count, 3] on the device = (data_ptr, numel, slot) -- bit-compatible with ppq_b200_tensor_desc
@@ -349,6 +434,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     register_more(m);
     // H100-native extras
     m.def("QuantizeTensor_toInt", QuantizeTensor_toInt, "QuantizeTensor_toInt");
+    m.def("QuantizeTensor_LT_Half", QuantizeTensor_LT_Half, "QuantizeTensor_LT_Half");
+    m.def("QuantizeTensor_LC_Half", QuantizeTensor_LC_Half, "QuantizeTensor_LC_Half");
+    m.def("QuantizeTensor_FT_Half", QuantizeTensor_FT_Half, "QuantizeTensor_FT_Half");
+    m.def("QuantizeTensor_FC_Half", QuantizeTensor_FC_Half, "QuantizeTensor_FC_Half");
+    m.def("Histogram_Asymmetric_T_Half", Histogram_Asymmetric_T_Half, "Histogram_Asymmetric_T_Half");
     m.def("Multi_QuantizeTensor_LC", Multi_QuantizeTensor_LC, "Multi_QuantizeTensor_LC");
     m.def("Multi_QuantizeTensor_LT", Multi_QuantizeTensor_LT, "Multi_QuantizeTensor_LT");
     m.def("MinMax_Init", MinMax_Init, "MinMax_Init");

@@ -214,13 +214,14 @@ class TorchExecutor:
     def _quantize_all_weights(self):
         """All activated per-channel linear weight configs that share (axis, range, rounding) are fake-quantised by ONE multi-tensor launch
         at the start of the forward (the per-module results are what the pre-forward hooks hand to the operations).  Falls back to one
-        launch per weight for anything else (FP8 weights, mixed policies)."""
+        launch per weight for anything else (FP8 weights, mixed policies, fp16 / bf16 weights: the table kernel reads fp32 only)."""
         from .calibration import MultiWeightQuantizer
         from .core import QuantizationProperty as P
         ops = [self.operations[n] for n in self._order]
         todo = [op for op in ops if op.weight_cfg is not None and QuantizationStates.is_activated(op.weight_cfg.state)
                 and op.weight_cfg.policy.has_property(P.LINEAR) and op.weight_cfg.policy.has_property(P.PER_CHANNEL)
-                and not op.weight_cfg.policy.has_property(P.DYNAMIC) and self._quant_fn is PPQuantFunction]
+                and not op.weight_cfg.policy.has_property(P.DYNAMIC) and self._quant_fn is PPQuantFunction
+                and op.module.weight.dtype == torch.float32]
         if len(todo) < 2: return {}
         c0 = todo[0].weight_cfg
         key0 = (c0.channel_axis, c0.quant_min, c0.quant_max, c0.rounding)
@@ -569,6 +570,10 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     trace: a list that receives (phase, batch index, host time, CUDA event, thread CPU time) before every batch and at the end of a phase --
     bench.py's e2e uses it to say whether a slow calibration was slow on the host or on the device, and where."""
     import time
+    half = sorted({str(p.dtype) for p in executor.model.parameters() if p.dtype != torch.float32})
+    if half:
+        raise TypeError(f'calibrate_arena: the multi-tensor collectors read fp32 tensors, this network has {", ".join(half)} parameters; '
+                        'calibrate it with RuntimeCalibrationPass (per-observer collectors, which take fp16 / bf16).')
     from .calibration import ArenaCalibrator, is_dense
     cfgs = executor.observed_configs()
     if graphs and method == 'percentile': raise ValueError('graphs=True needs static statistics buffers; the percentile observer keeps one row per batch')
@@ -686,7 +691,7 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
     def snr_all(fp, qt):
         out = []
         for n in names:
-            f, q = sample(fp[n]), sample(qt[n])
+            f, q = sample(fp[n]).float(), sample(qt[n]).float()            # fp16 / bf16 activations: the SNR is accumulated in fp32
             out.append((torch.pow(q - f, 2).sum(dim=-1) / (torch.pow(f, 2).sum(dim=-1) + 1e-7)).mean())
         return torch.stack(out)
 

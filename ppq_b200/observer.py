@@ -163,7 +163,10 @@ class TorchHistObserver(TorchMinMaxObserver):
         if self._phase == 'Detecting Minmax':
             return super().observe(value)
         if self._quant_cfg.policy.has_property(QuantizationProperty.ASYMMETRICAL):
-            CUDA.Histogram_Asymmetric_T(self._min, self._max, tensor=value, histogram=self._slot.hist)
+            if value.dtype in (torch.float16, torch.bfloat16):
+                _ext().Histogram_Asymmetric_T_Half(self._min, self._max, value, True, self._slot.hist)
+            else:
+                CUDA.Histogram_Asymmetric_T(self._min, self._max, tensor=value, histogram=self._slot.hist)
         elif self._quant_cfg.policy.has_property(QuantizationProperty.SYMMETRICAL):
             _ext().Histogram_T_DeviceScale(value, self._slot.hist_scale, True, self._slot.hist)
         else:
@@ -329,7 +332,8 @@ class DirectMSEObserver(BaseTensorObserver):
             raise PermissionError('Observer collector is empty, you should invoke observe function before render quantization config.')
         set_state(cfg, 'ACTIVATED')
         per_channel = cfg.policy.has_property(QuantizationProperty.PER_CHANNEL)
-        data = torch.cat(self._collector, dim=-1 if per_channel else 0).contiguous()
+        # fp16 / bf16 samples are scored on their exact fp32 upcast, so the choice is the one the fp32 path makes on x.float()
+        data = torch.cat(self._collector, dim=-1 if per_channel else 0).float().contiguous()
         n = data.shape[0] if per_channel else 1
         cand = torch.tensor(self.SCALE_CANDIDATES, dtype=torch.float32, device=data.device)
         saved_axis = cfg.channel_axis

@@ -20,14 +20,39 @@ def _require_cuda(tensor: torch.Tensor):
         raise PermissionError('ppq_b200 quantization functions require CUDA tensors (no CPU fallback exists in this package).')
 
 
+HALF_DTYPES = (torch.float16, torch.bfloat16)
+
+
+def _is_half(tensor: torch.Tensor) -> bool:
+    """fp16 / bf16 values go to the *_Half kernels: the fp32 result on the exact upcast, rounded once back to the input's dtype."""
+    return tensor.dtype in HALF_DTYPES
+
+
+def _linear_t(tensor, scales, offsets, quant_min, quant_max, rounding):
+    if _is_half(tensor):
+        return CUDA_COMPLIER.CUDA_EXTENSION.QuantizeTensor_LT_Half(tensor, scales, offsets, quant_min, quant_max, rounding)
+    return CUDA.LinearQuantize_T(tensor=tensor, scales=scales, offsets=offsets, minimum=quant_min, maximum=quant_max, rounding=rounding)
+
+
+def _linear_c(tensor, scales, offsets, channel_axis, quant_min, quant_max, rounding):
+    if _is_half(tensor):
+        return CUDA_COMPLIER.CUDA_EXTENSION.QuantizeTensor_LC_Half(tensor, scales, offsets, quant_min, quant_max, channel_axis, rounding)
+    return CUDA.LinearQuantize_C(tensor=tensor, scales=scales, offsets=offsets, channel_axis=channel_axis,
+                                 minimum=quant_min, maximum=quant_max, rounding=rounding)
+
+
+def _refuse_half(tensor: torch.Tensor, what: str):
+    if _is_half(tensor):
+        raise TypeError(f'{what} needs an fp32 tensor: its backward kernels do not take {tensor.dtype} (cast with .float()).')
+
+
 class TensorwiseLinearQuantImpl(Function):
     """linear.py:8-50 (CUDA branch :34-46)."""
     @staticmethod
     def forward(ctx, tensor, scales, offsets, quant_min: int, quant_max: int, rounding) -> torch.Tensor:
         _require_cuda(tensor)
         scales, offsets = scales.to(tensor.device), offsets.to(tensor.device)
-        return CUDA.LinearQuantize_T(tensor=tensor, scales=scales, offsets=offsets, minimum=quant_min, maximum=quant_max,
-                                     rounding=_rounding_value(rounding))
+        return _linear_t(tensor, scales, offsets, quant_min, quant_max, _rounding_value(rounding))
 
     @staticmethod
     def backward(ctx, dy: torch.Tensor):
@@ -40,8 +65,7 @@ class ChannelwiseLinearQuantImpl(Function):
     def forward(ctx, tensor, scales, offsets, channel_axis: int, quant_min: int, quant_max: int, rounding) -> torch.Tensor:
         _require_cuda(tensor)
         scales, offsets = scales.to(tensor.device), offsets.to(tensor.device)
-        return CUDA.LinearQuantize_C(tensor=tensor, scales=scales, offsets=offsets, channel_axis=channel_axis,
-                                     minimum=quant_min, maximum=quant_max, rounding=_rounding_value(rounding))
+        return _linear_c(tensor, scales, offsets, channel_axis, quant_min, quant_max, _rounding_value(rounding))
 
     @staticmethod
     def backward(ctx, dy: torch.Tensor):
@@ -55,6 +79,10 @@ class TensorwiseFloatingQuantImpl(Function):
                 rounding) -> torch.Tensor:
         _require_cuda(tensor)
         scales, offsets = scales.to(tensor.device), offsets.to(tensor.device)
+        if _is_half(tensor):
+            if exponet_bits <= 0: raise ValueError('Floating Quantization requires exponent > 0')
+            return CUDA_COMPLIER.CUDA_EXTENSION.QuantizeTensor_FT_Half(tensor.contiguous(), scales, offsets, exponet_bits, mantissa_bits,
+                                                                       quant_min, quant_max, _rounding_value(rounding))
         return CUDA.FloatingQuantize_T(tensor=tensor, scales=scales, offsets=offsets, exponent=exponet_bits,
                                        mantissa=mantissa_bits, minimum=quant_min, maximum=quant_max,
                                        rounding=_rounding_value(rounding))
@@ -71,6 +99,10 @@ class ChannelwiseFloatingQuantImpl(Function):
                 quant_max: float, rounding) -> torch.Tensor:
         _require_cuda(tensor)
         scales, offsets = scales.to(tensor.device), offsets.to(tensor.device)
+        if _is_half(tensor):
+            if exponet_bits <= 0: raise ValueError('Floating Quantization requires exponent > 0')
+            return CUDA_COMPLIER.CUDA_EXTENSION.QuantizeTensor_FC_Half(tensor.contiguous(), scales, offsets, exponet_bits, mantissa_bits,
+                                                                       quant_min, quant_max, channel_axis, _rounding_value(rounding))
         return CUDA.FloatingQuantize_C(tensor=tensor, scales=scales, offsets=offsets, channel_axis=channel_axis,
                                        exponent=exponet_bits, mantissa=mantissa_bits, minimum=quant_min, maximum=quant_max,
                                        rounding=_rounding_value(rounding))
@@ -116,12 +148,12 @@ def PPQDyamicLinearQuantFunction(tensor: torch.Tensor, config: TensorQuantizatio
         ext.MinMax_Init(mins, maxs)
         ext.MinMax_C(tensor, config.channel_axis, mins, maxs)
         scales, offsets = ext.MinMax_To_Scale_Offset(mins, maxs, 1, config.quant_min, config.quant_max, sym, pow2, min_scale)
-        return CUDA.LinearQuantize_C(tensor, scales, offsets, config.channel_axis, config.quant_min, config.quant_max, rounding)
+        return _linear_c(tensor, scales, offsets, config.channel_axis, config.quant_min, config.quant_max, rounding)
     mm = torch.empty(2, dtype=torch.float32, device=tensor.device)
     ext.MinMax_Init(mm[0:1], mm[1:2])
     ext.MinMax_T(tensor, mm)
     scales, offsets = ext.MinMax_To_Scale_Offset(mm[0:1], mm[1:2], 1, config.quant_min, config.quant_max, sym, pow2, min_scale)
-    return CUDA.LinearQuantize_T(tensor, scales, offsets, config.quant_min, config.quant_max, rounding)
+    return _linear_t(tensor, scales, offsets, config.quant_min, config.quant_max, rounding)
 
 
 def PPQFloatingQuantFunction(tensor: torch.Tensor, config: TensorQuantizationConfig) -> torch.Tensor:
@@ -190,6 +222,7 @@ class CuLSQ_LT(Function):
     @staticmethod
     def forward(ctx, tensor, scales, offsets, quant_min: int, quant_max: int, rounding) -> torch.Tensor:
         _require_cuda(tensor)
+        _refuse_half(tensor, 'CuLSQ_LT')
         r = _rounding_value(rounding)
         quantized = CUDA.LinearQuantize_T(tensor=tensor, scales=scales, offsets=offsets, minimum=quant_min, maximum=quant_max, rounding=r)
         ctx.save_for_backward(tensor, scales, offsets)
@@ -209,6 +242,7 @@ class CuLSQ_LC(Function):
     @staticmethod
     def forward(ctx, tensor, scales, offsets, channel_axis: int, quant_min: int, quant_max: int, rounding) -> torch.Tensor:
         _require_cuda(tensor)
+        _refuse_half(tensor, 'CuLSQ_LC')
         r = _rounding_value(rounding)
         quantized = CUDA.LinearQuantize_C(tensor=tensor, scales=scales, offsets=offsets, channel_axis=channel_axis,
                                           minimum=quant_min, maximum=quant_max, rounding=r)
