@@ -217,7 +217,7 @@ PPQ_B200_API int ppq_b200_multi_histogram_t(const ppq_b200_tensor_desc *descs, i
  * then owned by this function) makes consecutive calls on the same slots speculative: keys beyond the thresholds remembered from the
  * previous call are compacted during the first pass, and when they contain the requested order statistics (the usual case for consecutive
  * calibration batches of one activation) the tensor is read ONCE.  A wrong guess only costs the regular second pass; results are always
- * the exact order statistics. */
+ * the exact order statistics.  An entry with n = 0 has no order statistics: its two output values and its guess words are left as they are. */
 PPQ_B200_API int64_t ppq_b200_multi_quantile_workspace_bytes(int count, int64_t cap);
 PPQ_B200_API int64_t ppq_b200_quantile_guess_words(void);
 PPQ_B200_API int ppq_b200_quantile_guess_init(uint32_t *guess, int64_t slots, void *stream);

@@ -93,7 +93,10 @@ def lib():
         L.ora_compute_mse_loss.argtypes = [_P, _I64, _I32, _I32, _I32]
         L.ora_minmax_t.argtypes = [_P, _I64, _P, _P]
         L.ora_minmax_c.argtypes = [_P, _I64, _I64, _I32, _P, _P]
-        L.ora_quantile_t.argtypes = [_P, _I64, _F, _P]
+        L.ora_select_t.argtypes = [_P, _I64, _P, _I32, _I32, _P]
+        L.ora_quantile_ranks.argtypes = [_I64, _F, _P]
+        L.ora_quantile_t.argtypes = [_P, _I64, _F, _I32, _P]
+        L.ora_isotone_t.argtypes = [_P, _I64, _I32, _P]
         L.ora_linear_quant_backward.restype = _F
         L.ora_linear_quant_backward.argtypes = [_P, _P, _I64, _I64, _I32, _I32, _P, _P, _I32, _I32, _I32, _P, _P]
         L.ora_float_quant_backward.restype = _F
@@ -271,9 +274,38 @@ def minmax_c(x, axis):
     return lo, hi
 
 
-def quantile_t(x, q):
+SEL_DEVICE, SEL_REFERENCE = 0, 1
+_SEMANTICS = {'device': SEL_DEVICE, 'reference': SEL_REFERENCE}
+
+
+def select_t(x, ranks, semantics='device'):
+    """The elements at ascending ranks `ranks` of an order-key sort of `x` (ppq_oracle.c, `ora_select_t`).  'device': one key per bit
+    pattern (-0 < +0, NaNs ordered by sign and payload), as the radix select; 'reference': -0 and +0 share a key and equal keys keep
+    their input order, as thrust::sort."""
+    x = _f32(x).reshape(-1); r = np.ascontiguousarray(ranks, dtype=np.int64).reshape(-1)
+    assert x.size > 0 and ((r >= 0) & (r < x.size)).all()
+    out = np.zeros(r.size, np.float32)
+    lib().ora_select_t(x.ctypes.data, x.size, r.ctypes.data, r.size, _SEMANTICS[semantics], out.ctypes.data)
+    return out
+
+
+def quantile_ranks(n, q):
+    """(clip(rn(n q)), clip(rn(n (1 - q)))) in fp32 arithmetic, as _Quantile_T computes them (sort.cu:13-19)."""
+    r = np.zeros(2, np.int64)
+    lib().ora_quantile_ranks(int(n), float(np.float32(q)), r.ctypes.data)
+    return int(r[0]), int(r[1])
+
+
+def quantile_t(x, q, semantics='device'):
     x = _f32(x); out = np.zeros(2, np.float32)
-    lib().ora_quantile_t(x.ctypes.data, x.size, float(np.float32(q)), out.ctypes.data)
+    lib().ora_quantile_t(x.ctypes.data, x.size, float(np.float32(q)), _SEMANTICS[semantics], out.ctypes.data)
+    return out
+
+
+def isotone_t(x, semantics='device'):
+    """Isotone_T: {sorted[n-1], sorted[n-2], sorted[0], sorted[1]}, four copies of x[0] when n == 1 (sort.cu:23-40)."""
+    x = _f32(x); out = np.zeros(4, np.float32)
+    lib().ora_isotone_t(x.ctypes.data, x.size, _SEMANTICS[semantics], out.ctypes.data)
     return out
 
 

@@ -6,9 +6,9 @@
 //                               TorchPercentileObserver, ppq/quantization/observer/range.py:312-403, is the reference's default observer).
 //   ppq_b200_isotone_t          replaces Isotone_T (sort.cu:23-40, 61-73): sorted[n-1], sorted[n-2], sorted[0], sorted[1].
 //
-// MSD radix *select* on the order-preserving 32-bit key of each float (the same total order thrust's radix sort uses:
-// -NaN < -inf < ... < -0 == +0 < ... < +inf < +NaN; the two zeros share one key, see order_key), digits of 11 + 11 + 10 bits, both
-// requested ranks resolved together.
+// MSD radix *select* on the order-preserving 32-bit key of each float (the order thrust's radix sort uses:
+// -NaN < -inf < ... < -0 < +0 < ... < +inf < +NaN, except that thrust gives the two zeros one key, see order_key), digits of 11 + 11 + 10
+// bits, both requested ranks resolved together.
 //
 //   pass 0   streams the tensor once (4 B/element): 2048-bin histogram of the top digit, shared-memory privatised.  The scan that ends the
 //            pass knows the population of the bucket each rank fell into.
@@ -602,6 +602,7 @@ select_finish_kernel(const SelectState *__restrict__ states, const uint32_t *__r
     __shared__ unsigned long long s_before, s_cnt;
     const int tensor = blockIdx.x >> 1, r = blockIdx.x & 1;
     const SelectState *st = states + tensor;
+    if (descs && descs[tensor].n <= 0) return;                         // an empty table entry has no order statistics: its slot and guess stay as they are
     float *dst = out + (descs ? (int64_t)descs[tensor].slot : 0) * out_stride + r;
     unsigned int key = st->prefix[r];
     if (st->mode[r] == kModeCompact) {
@@ -721,7 +722,7 @@ static int select_two(const T *x, int64_t n, int q_mode, float q, long long r0, 
     } else {
         switch ((variant_of(kVarSelect) >> 3) & 7) {                             // ... and of pass 1
         case 1: select_pass_kernel<1, kFilterThreads, 2><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
-        case 2: select_pass_kernel<1, 512, 4, true, 3><<<grid_filter(n) / 2, 512, 0, s>>>(x, n, st, bufs, cap); break;
+        case 2: select_pass_kernel<1, 512, 4, true, 3><<<grid_filter(n) > 1 ? grid_filter(n) / 2 : 1, 512, 0, s>>>(x, n, st, bufs, cap); break;
         case 3: select_pass_kernel<1, 1024, 2, true, 2><<<grid_pass0(n), 1024, 0, s>>>(x, n, st, bufs, cap); break;
         case 4: select_pass_kernel<1, kFilterThreads, 4, false><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap); break;
         default: select_pass_kernel<1, kFilterThreads><<<grid_filter(n), kFilterThreads, 0, s>>>(x, n, st, bufs, cap);

@@ -133,7 +133,8 @@ def expected(oracle, algo: str, spec: dict, xs):
     if algo == 'minmax':
         return oracle.minmax_to_scale_offset(vmin, vmax, qmin, qmax, sym, pow2, thr, ieee=True)
     if algo == 'percentile':
-        pairs = torch.tensor(np.stack([oracle.quantile_t(x, 0.9999) for x in xs]), dtype=torch.float32, device='cuda')
+        # the select's key order (oracle device semantics): a +NaN is the largest element, so a NaN batch makes the mean and the scale NaN
+        pairs = torch.tensor(np.stack([oracle.quantile_t(x, 0.9999, 'device') for x in xs]), dtype=torch.float32, device='cuda')
         mean = pairs.mean(dim=0).cpu()                             # range.py:369: the fp32 mean over [batches, 2] on the tensors' device
         return oracle.minmax_to_scale_offset(float(mean[1]), float(mean[0]), qmin, qmax, sym, pow2, thr, ieee=True)
     bins = spec.get('detail', {}).get(KL_BINS, 4096) if algo == 'kl' else 2048
@@ -161,7 +162,6 @@ def test_configs_through_hook_and_arena_paths(ext, oracle, name, algo):
     spec = CONFIGS[name]
     arena_refuses = (algo == 'mse' and not spec['sym']) or spec.get('detail', {}).get(KL_BINS, 0) > 12287
     for j, kind in enumerate(DATA):
-        if kind == 'nan' and algo == 'percentile': continue        # the select's NaN order is defined by neither the oracle nor a recording
         host = batches_of(kind, 1000 + 17 * j)
         data = [torch.from_numpy(x).cuda() for x in host]
         ex_hook, ex_arena = executor_with(spec), executor_with(spec)
