@@ -88,8 +88,8 @@ PPQ_B200_API int ppq_b200_linear_quant_c_toint_dt(const void *x, int dtype, void
 /* Every per-channel weight of a network in ONE launch (the executor re-quantises all Conv/Gemm weights on every forward until
  * they are baked: ppq/executor/torch.py:516-518; ParameterBakingPass, optim/baking.py:34-47).  Descriptors in DEVICE memory. */
 typedef struct {
-    const float *x;        /* fp32 weight                     */
-    float       *y;        /* fake-quantised output (!= x)    */
+    const float *x;        /* weight (fp32; the table's type in the `_dt` entry) */
+    float       *y;        /* fake-quantised output (!= x), same type as x */
     const float *scale;    /* [C] */
     const float *offset;   /* [C] */
     int64_t      n;        /* elements                        */
@@ -100,6 +100,11 @@ typedef struct {
 /* count <= 4096 tensors per call, every n <= 2^31 - 1; max_n = the largest n of the table (sizes the grid). */
 PPQ_B200_API int ppq_b200_multi_linear_quant_c(const ppq_b200_lc_desc *descs, int count, int64_t max_n,
                                                int qmin, int qmax, int rounding, void *stream);
+/* The same for a table whose weights all have element type `dtype`: `x` and `y` of every descriptor point at elements of that type
+ * (the struct keeps its layout; the element type is one per table, not per descriptor), `y` holds the fp32 result on x.float()
+ * rounded once to nearest even -- what ppq_b200_linear_quant_c_dt writes for that weight.  scale / offset stay fp32. */
+PPQ_B200_API int ppq_b200_multi_linear_quant_c_dt(const ppq_b200_lc_desc *descs, int count, int64_t max_n, int dtype,
+                                                  int qmin, int qmax, int rounding, void *stream);
 
 /* QuantizeTensor_LT (linear.cu:88-130) for a table of tensors in ONE launch, each with its own (scale, offset): the per-tensor
  * activation configs of a quantised graph (executor/torch.py:516-518, 541-543 call the op ~100x per forward on tensors of a few hundred KB,
@@ -195,9 +200,12 @@ PPQ_B200_API int ppq_b200_isotone_t(const float *x, int64_t n, float *out4, void
  *   minmax arena: float[2 * slots]  ({min, max} per slot);   hist arena: int32[slots * bins];
  *   hist_scale arena: float[slots].
  * Both keep a prefix of the table's sizes in shared memory ((count + 1) x 8 bytes next to a 64 KB staging ring and, for the histogram,
- * (bins + 1) x 4 bytes of private counters); a table that does not fit the device's shared memory per block is rejected. */
+ * (bins + 1) x 4 bytes of private counters); a table that does not fit the device's shared memory per block is rejected.
+ * The `_dt` entries take a table whose tensors all have element type `dtype` (one per table, not per descriptor: `x` of every
+ * descriptor points at elements of that type, which may start at any element-aligned address); every statistic equals, bit for bit,
+ * what the fp32 entry writes for the same table over the upcasts x.float().  A mixed set of tensors is served by one call per type. */
 typedef struct {
-    const float *x;      /* device pointer to the tensor */
+    const float *x;      /* device pointer to the tensor (elements of the table's type in the `_dt` entries) */
     int64_t      n;      /* elements */
     int32_t      slot;   /* statistics slot */
     int32_t      pad_;
@@ -208,6 +216,11 @@ PPQ_B200_API int ppq_b200_multi_minmax_t(const ppq_b200_tensor_desc *descs, int 
 PPQ_B200_API int ppq_b200_multi_histogram_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n,
                                             const float *hist_scale_arena, int clip_outliers,
                                             int32_t *hist_arena, int64_t bins, void *stream);
+PPQ_B200_API int ppq_b200_multi_minmax_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype,
+                                            float *minmax_arena, void *stream);
+PPQ_B200_API int ppq_b200_multi_histogram_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype,
+                                               const float *hist_scale_arena, int clip_outliers,
+                                               int32_t *hist_arena, int64_t bins, void *stream);
 /* Quantile_T (sort.cu:6-20, 42-59) for a table of tensors, one launch per pass: what TorchPercentileObserver.observe
  * (ppq/quantization/observer/range.py:338-349) asks for once per observed tensor and batch.  Tensor i writes
  * out[slot_i * out_stride + {0, 1}] = {sorted[clip(rn(n q))], sorted[clip(rn(n (1 - q)))]}.  `cap` = keys of a selected bucket the
@@ -223,6 +236,9 @@ PPQ_B200_API int64_t ppq_b200_quantile_guess_words(void);
 PPQ_B200_API int ppq_b200_quantile_guess_init(uint32_t *guess, int64_t slots, void *stream);
 PPQ_B200_API int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float q,
                                            float *out, int64_t out_stride, void *workspace, int64_t cap, uint32_t *guess, void *stream);
+/* the same for a table of element type `dtype`: workspace size, `cap` and the guess words are those of the fp32 entry. */
+PPQ_B200_API int ppq_b200_multi_quantile_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype, float q,
+                                              float *out, int64_t out_stride, void *workspace, int64_t cap, uint32_t *guess, void *stream);
 
 /* ---- scale / offset search on the device ---------------------------------------------------------------------- */
 /* replaces minmax_to_scale_offset, ppq/quantization/observer/range.py:22-75, vectorised over `count` ranges

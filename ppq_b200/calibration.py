@@ -135,6 +135,19 @@ def shared_stager(device, columns: int) -> DescriptorStager:
     return _STAGERS[key]
 
 
+TABLE_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def descriptor_rows_by_dtype(tensors: Sequence[torch.Tensor], slots: Sequence[int]) -> Dict[torch.dtype, tuple]:
+    """The (data_ptr, numel, slot) rows of a collector table, one tuple of rows per element type: a table carries raw pointers and one
+    element type, so a mixed set of tensors (an fp32 network under autocast) becomes one table -- one launch -- per dtype present.  Every
+    tensor keeps its slot; groups appear in the order their dtype is first met and rows keep the order of `tensors`."""
+    groups: Dict[torch.dtype, list] = {}
+    for t, i in zip(tensors, slots):
+        groups.setdefault(t.dtype, []).append((t.data_ptr(), t.numel(), i))
+    return {dtype: tuple(rows) for dtype, rows in groups.items()}
+
+
 ARENA_MAX_HIST_BINS = 12287          # the multi-tensor histogram keeps (bins + 1) private counters in 48 KB of shared memory
 
 
@@ -146,12 +159,14 @@ class ArenaCalibrator:
                               batches in sample order                        -> MinMax_To_Scale_Offset   (range.py:312-403)
     All T tensors share one per-tensor config: range (quant_min, quant_max, num_of_bits), symmetrical, power_of_2 and min_scale.  The
     histogram of both two-phase methods is symmetric (|x| binned from 0), so asymmetric 'kl' / 'mse' are refused, as are more than
-    ARENA_MAX_HIST_BINS bins."""
+    ARENA_MAX_HIST_BINS bins.
+    half_inputs=True also takes fp16 / bf16 tensors (the *_Half table kernels: the same statistics, bit for bit, as on x.float()); the
+    tensors of one `observe` call may mix element types and are served by one launch per type present."""
 
     def __init__(self, num_tensors: int, device, bins: int = None, num_of_bits: int = 8,
                  quant_min: int = -128, quant_max: int = 127, power_of_2: bool = False, min_scale: float = OBSERVER_MIN_SCALE,
                  method: str = 'kl', group=None, percentile: float = OBSERVER_PERCENTILE, select_cap: int = 1 << 16,
-                 symmetrical: bool = True):
+                 symmetrical: bool = True, half_inputs: bool = False):
         from .ffi import extension
         if method not in ('kl', 'minmax', 'mse', 'percentile'):
             raise ValueError(f"ArenaCalibrator: unknown observer algorithm {method!r} (expected 'kl', 'minmax', 'mse' or 'percentile')")
@@ -168,7 +183,7 @@ class ArenaCalibrator:
         self.T, self.bins, self.device, self.group = num_tensors, bins, torch.device(device), group
         self.num_of_bits, self.quant_min, self.quant_max = num_of_bits, quant_min, quant_max
         self.power_of_2, self.min_scale, self.method, self.symmetrical = power_of_2, min_scale, method, symmetrical
-        self.percentile, self.select_cap = percentile, select_cap
+        self.percentile, self.select_cap, self.half_inputs = percentile, select_cap, half_inputs
         self.minmax = torch.empty(num_tensors, 2, dtype=torch.float32, device=self.device)
         two_phase = method in ('kl', 'mse')
         self.hist = torch.zeros(num_tensors, bins if two_phase else 1, dtype=torch.int32, device=self.device)
@@ -193,11 +208,12 @@ class ArenaCalibrator:
         if slots is None:
             assert len(tensors) == self.T, f'expected {self.T} tensors per forward, got {len(tensors)}'
             slots = range(self.T)
+        allowed = TABLE_DTYPES if self.half_inputs else (torch.float32,)
         for t in tensors:
-            if not (t.is_cuda and t.dtype == torch.float32 and is_dense(t)):
-                raise RuntimeError('ArenaCalibrator needs dense (contiguous or channels_last) fp32 CUDA tensors')
-        key = tuple((t.data_ptr(), t.numel(), i) for t, i in zip(tensors, slots))
-        return self._stager.get(key), max(k[1] for k in key)
+            if not (t.is_cuda and t.dtype in allowed and is_dense(t)):
+                raise RuntimeError('ArenaCalibrator needs dense (contiguous or channels_last) ' +
+                                   ('fp32, fp16 or bf16' if self.half_inputs else 'fp32') + ' CUDA tensors')
+        return [(dtype, self._stager.get(rows), max(r[1] for r in rows)) for dtype, rows in descriptor_rows_by_dtype(tensors, slots).items()]
 
     def begin_batch(self):
         """Call before every forward: the percentile observer keeps one {upper, lower} row per batch (range.py:349), whatever number of
@@ -211,28 +227,35 @@ class ArenaCalibrator:
 
     @torch.no_grad()
     def observe(self, tensors: Sequence[torch.Tensor], slots: Optional[Sequence[int]] = None):
-        """One multi-tensor launch over `tensors`; tensor j accumulates into arena slot slots[j] (default: j)."""
+        """One multi-tensor launch per element type present in `tensors` (one for an all-fp32 or all-half forward, two under autocast);
+        tensor j accumulates into arena slot slots[j] (default: j)."""
         if len(tensors) == 0: return
-        descs, max_n = self._descs(tensors, slots)
+        groups = self._descs(tensors, slots)
         if self.method == 'percentile':
-            need = self.ext.Multi_Quantile_Workspace_Bytes(len(tensors), self.select_cap)
+            need = self.ext.Multi_Quantile_Workspace_Bytes(len(tensors), self.select_cap)      # sized for the whole set: every group fits
             if self._select_ws is None or self._select_ws.numel() < need:
                 self._select_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-            self.ext.Multi_Quantile_T(descs, max_n, self.percentile, self._batch_quantiles(), 2, self._select_ws, self.select_cap, self._select_guess)
-            self.launches += 5
-            return
-        if self.phase == 1:
-            self.ext.Multi_MinMax_T(descs, max_n, self.minmax)
-        else:
-            self.ext.Multi_Histogram_T(descs, max_n, self.hist_scale, True, self.hist, self.bins)
-        self.launches += 1
+        for dtype, descs, max_n in groups:
+            half = (dtype,) if dtype != torch.float32 else ()
+            ext, suffix = self.ext, '_Half' if half else ''
+            if self.method == 'percentile':
+                getattr(ext, 'Multi_Quantile_T' + suffix)(descs, max_n, *half, self.percentile, self._batch_quantiles(), 2, self._select_ws,
+                                                          self.select_cap, self._select_guess)
+                self.launches += 5
+            elif self.phase == 1:
+                getattr(ext, 'Multi_MinMax_T' + suffix)(descs, max_n, *half, self.minmax)
+                self.launches += 1
+            else:
+                getattr(ext, 'Multi_Histogram_T' + suffix)(descs, max_n, *half, self.hist_scale, True, self.hist, self.bins)
+                self.launches += 1
 
     @torch.no_grad()
     def observe_one(self, index: int, tensor: torch.Tensor):
         """Immediate single-tensor collection into slot `index` (used while a forward is running: later in-place ops of the
         network may overwrite the tensor, so it cannot wait for the end-of-forward multi-tensor launch)."""
         if self.method == 'percentile':
-            self._batch_quantiles()[index].copy_(self.ext.Quantile_T(tensor, self.percentile))
+            quantile = self.ext.Quantile_T if tensor.dtype == torch.float32 else self.ext.Quantile_T_Half
+            self._batch_quantiles()[index].copy_(quantile(tensor, self.percentile))
             self.launches += 5
             return
         if self.phase == 1:
@@ -456,17 +479,24 @@ class MultiWeightQuantizer:
     """All per-channel weights of a network fake-quantised by ONE launch (Multi_QuantizeTensor_LC), or -- with channel_axis=None -- any list
     of per-tensor quantised tensors, each with its own (scale, offset), by ONE Multi_QuantizeTensor_LT launch.  The executor re-quantises
     every Conv/Gemm weight on each forward until ParameterBakingPass freezes them (executor/torch.py:516-518); with ~54 small
-    tensors per ResNet-50 forward that is launch-latency, not bandwidth -- one descriptor table turns it into one kernel."""
+    tensors per ResNet-50 forward that is launch-latency, not bandwidth -- one descriptor table turns it into one kernel.
+    half_inputs=True takes per-channel weights that are all fp16 or all bf16 (Multi_QuantizeTensor_LC_Half: outputs in the weights' dtype,
+    the values QuantizeTensor_LC_Half returns per weight); scales and offsets stay fp32.  The per-tensor table is fp32 only."""
 
     def __init__(self, weights: Sequence[torch.Tensor], scales: Sequence[torch.Tensor], offsets: Sequence[torch.Tensor],
-                 channel_axis: Optional[int] = 0, quant_min: int = -128, quant_max: int = 127, rounding: int = 0):
+                 channel_axis: Optional[int] = 0, quant_min: int = -128, quant_max: int = 127, rounding: int = 0,
+                 half_inputs: bool = False):
         from .ffi import extension
         self.ext = extension()
         self.quant_min, self.quant_max, self.rounding = quant_min, quant_max, rounding
         self.per_tensor = channel_axis is None
         # the descriptor table carries raw pointers and the table kernels read and write fp32: any other dtype must never reach them
-        bad = sorted({str(t.dtype) for t in list(weights) + list(scales) + list(offsets) if t.dtype != torch.float32})
-        if bad: raise TypeError(f'MultiWeightQuantizer takes fp32 weights, scales and offsets only, got {", ".join(bad)}.')
+        self.dtype = weights[0].dtype if (half_inputs and not self.per_tensor and weights[0].dtype in TABLE_DTYPES) else torch.float32
+        bad = sorted({str(t.dtype) for t in weights if t.dtype != self.dtype} |
+                     {str(t.dtype) for t in list(scales) + list(offsets) if t.dtype != torch.float32})
+        if bad and not half_inputs: raise TypeError(f'MultiWeightQuantizer takes fp32 weights, scales and offsets only, got {", ".join(bad)}.')
+        if bad: raise TypeError('MultiWeightQuantizer(half_inputs=True) takes per-channel weights of ONE dtype (fp32, fp16 or bf16) with fp32 '
+                                f'scales and offsets, got {", ".join(bad)} next to {self.dtype} weights.')
 
         def rows_in_storage_order(w):
             # axis-0 channels of a dense tensor whose dim 0 is outermost in memory (NCHW or channels_last weights): the storage already is [C, epc]
@@ -495,6 +525,10 @@ class MultiWeightQuantizer:
 
     @torch.no_grad()
     def __call__(self) -> List[torch.Tensor]:
+        if self.dtype != torch.float32:
+            for table in self._tables:
+                self.ext.Multi_QuantizeTensor_LC_Half(table, self.max_n, self.dtype, self.quant_min, self.quant_max, self.rounding)
+            return self.outputs
         launch = self.ext.Multi_QuantizeTensor_LT if self.per_tensor else self.ext.Multi_QuantizeTensor_LC
         for table in self._tables:
             launch(table, self.max_n, self.quant_min, self.quant_max, self.rounding)

@@ -374,12 +374,15 @@ histogram_dscale_kernel(const T *__restrict__ x, int64_t n, const float *__restr
 }
 
 // ---- multi-tensor collectors: one streaming engine ------------------------------------------------------------------------
-// Each CTA owns one contiguous span of the concatenation of all tensors (cut points inside a tensor rounded up to a multiple of 4
-// elements, the same way by both neighbours), so per-tensor state is set up and published (#CTAs + #tensors) times per launch.
+// Each CTA owns one contiguous span of the concatenation of all tensors (cut points inside a tensor rounded up to a multiple of one
+// 16-byte vector -- 4 fp32 or 8 fp16 / bf16 elements -- the same way by both neighbours), so per-tensor state is set up and published
+// (#CTAs + #tensors) times per launch.  The element type T is one per table: every descriptor's `x` points at elements of that type.
 // Warp-specialised CTA: one producer lane walks the CTA's pieces (tensor t, elements [a, b)) and issues 1-D cp.async.bulk copies of
 // their 16-byte-aligned bodies into a ring of kRingStages tiles (full / empty mbarriers); the consumer warps walk the same pieces,
-// apply Op to every element of each tile from shared memory, and handle the (at most 3 + 3) unaligned head / tail elements of a piece
-// with plain loads.  Copies keep flowing while the consumers bin, flush or wait at a piece boundary.
+// apply Op to every element of each tile from shared memory (half elements are unpacked to fp32 in registers: the ring moves bytes, a
+// 16 KB stage is 4096 floats or 8192 halves), and handle the unaligned head / tail elements of a piece (at most 3 + 3 floats, 7 + 7
+// halves: a half tensor may start at any 2-byte offset) with plain loads.  Copies keep flowing while the consumers bin, flush or wait
+// at a piece boundary.
 constexpr int kRingConsumers = 512;                  // 16 consumer warps
 constexpr int kRingThreads = kRingConsumers + 32;    // + the producer warp
 constexpr int kRingTileVec = 1024;                   // float4 per tile (16 KB): two per consumer thread
@@ -449,9 +452,11 @@ struct HistOp {
 __host__ __device__ inline size_t ring_prefix_offset() { return (size_t)kRingStages * kRingTileVec * 16 + 2 * kRingStages * sizeof(uint64_t); }
 __host__ __device__ inline size_t ring_op_offset(int count) { return ring_prefix_offset() + (size_t)(count + 1) * sizeof(int64_t); }
 
-template <class Op>
+template <class Op, class T = float>
 __global__ void __launch_bounds__(kRingThreads, 2)
 multi_stream_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, typename Op::Args args) {
+    constexpr int64_t kVecElems = 16 / sizeof(T);                      // elements per 16-byte vector
+    constexpr int kVecShift = sizeof(T) == 4 ? 2 : 3;
     extern __shared__ __align__(128) unsigned char smem[];
     float4 *ring = reinterpret_cast<float4 *>(smem);
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + (size_t)kRingStages * kRingTileVec * 16), *empty = full + kRingStages;
@@ -480,31 +485,34 @@ multi_stream_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, t
     __syncthreads();
     const int64_t total = prefix[count];
     int64_t span = (total + gridDim.x - 1) / gridDim.x;
-    span = (span + 3) & ~(int64_t)3;
+    span = (span + kVecElems - 1) & ~(kVecElems - 1);
     const int64_t s0 = (int64_t)blockIdx.x * span, s1 = (s0 + span) < total ? (s0 + span) : total;
     if (s0 >= total) return;                                           // uniform per CTA
     int t_first;                                                       // first tensor overlapping [s0, s1): binary search
     { int lo = 0, hi = count - 1; while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (prefix[mid] <= s0) lo = mid; else hi = mid - 1; } t_first = lo; }
 
-    // The pieces of this CTA, walked identically by the producer and the consumers.  body = [ia, ia + 4 nv) is 16-byte aligned.
+    // The pieces of this CTA, walked identically by the producer and the consumers.  body = [ia, ia + kVecElems nv) is 16-byte aligned.
     auto for_each_piece = [&](auto &&f) {
         for (int t = t_first; t < count && prefix[t] < s1; t++) {
             const ppq_b200_tensor_desc d = descs[t];
             int64_t a = s0 - prefix[t]; if (a < 0) a = 0;
             int64_t b = s1 - prefix[t]; if (b > d.n) b = d.n;
-            a = (a + 3) & ~(int64_t)3; if (a > d.n) a = d.n;
-            if (b < d.n) b = (b + 3) & ~(int64_t)3; if (b > d.n) b = d.n;
+            a = (a + kVecElems - 1) & ~(kVecElems - 1); if (a > d.n) a = d.n;
+            if (b < d.n) b = (b + kVecElems - 1) & ~(kVecElems - 1); if (b > d.n) b = d.n;
             if (b <= a) continue;
-            int64_t ia = a + (int64_t)((4u - (uint32_t)((reinterpret_cast<uintptr_t>(d.x + a) >> 2) & 3u)) & 3u);
+            const T *x = reinterpret_cast<const T *>(d.x);
+            int64_t ia;
+            if constexpr (sizeof(T) == 4) ia = a + (int64_t)((4u - (uint32_t)((reinterpret_cast<uintptr_t>(x + a) >> 2) & 3u)) & 3u);
+            else ia = a + head_elems(x + a);
             if (ia > b) ia = b;
-            f(d, a, b, ia, (b - ia) >> 2);
+            f(d, x, a, b, ia, (b - ia) >> kVecShift);
         }
     };
     if (threadIdx.x >= kRingConsumers) {
         if (threadIdx.x == kRingConsumers) {                           // producer: one lane
             uint32_t k = 0;
-            for_each_piece([&](const ppq_b200_tensor_desc &d, int64_t, int64_t, int64_t ia, int64_t nv) {
-                const float4 *src = reinterpret_cast<const float4 *>(d.x + ia);
+            for_each_piece([&](const ppq_b200_tensor_desc &, const T *x, int64_t, int64_t, int64_t ia, int64_t nv) {
+                const float4 *src = reinterpret_cast<const float4 *>(x + ia);
                 for (int64_t v0 = 0; v0 < nv; v0 += kRingTileVec, k++) {
                     const uint32_t s = k % kRingStages, bytes = (uint32_t)((nv - v0) < kRingTileVec ? (nv - v0) : kRingTileVec) * 16u;
                     if (k >= kRingStages) ring_wait(empty + s, ((k / kRingStages) - 1) & 1);
@@ -518,12 +526,12 @@ multi_stream_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, t
     }
     Op op(args, smem + ring_op_offset(count));
     uint32_t k = 0;
-    for_each_piece([&](const ppq_b200_tensor_desc &d, int64_t a, int64_t b, int64_t ia, int64_t nv) {
+    for_each_piece([&](const ppq_b200_tensor_desc &d, const T *x, int64_t a, int64_t b, int64_t ia, int64_t nv) {
         op.begin(d);
-        const int64_t ib = ia + 4 * nv;                                // ragged head [a, ia) and tail [ib, b): at most 3 + 3 elements
+        const int64_t ib = ia + kVecElems * nv;                        // ragged head [a, ia) and tail [ib, b): < kVecElems elements each
         const int i = (int)threadIdx.x, head = (int)(ia - a);
-        if (i < head) op.add(ld_stream1(d.x + a + i));
-        else if (i < head + (int)(b - ib)) op.add(ld_stream1(d.x + ib + (i - head)));
+        if (i < head) op.add(ld_stream1_f(x + a + i));
+        else if (i < head + (int)(b - ib)) op.add(ld_stream1_f(x + ib + (i - head)));
         for (int64_t v0 = 0; v0 < nv; v0 += kRingTileVec, k++) {
             const uint32_t s = k % kRingStages;
             const int cnt = (int)((nv - v0) < kRingTileVec ? (nv - v0) : kRingTileVec);
@@ -532,7 +540,13 @@ multi_stream_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, t
 #pragma unroll
             for (int j = 0; j < kRingTileVec / kRingConsumers; j++) {
                 const int vi = i + j * kRingConsumers;
-                if (vi < cnt) op.add4(tile[vi]);
+                if constexpr (sizeof(T) == 4) {
+                    if (vi < cnt) op.add4(tile[vi]);
+                } else if (vi < cnt) {
+                    float4 lo, hi;
+                    unpack8<T>(reinterpret_cast<const uint4 *>(tile)[vi], lo, hi);
+                    op.add4(lo); op.add4(hi);
+                }
             }
             __syncwarp();
             if ((i & 31) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(empty + s)) : "memory");
@@ -616,7 +630,7 @@ static int launch_hist_half(const T *x, int64_t n, const BinParams &bin, int64_t
 
 // Two CTAs per SM when the ring, the prefix and the Op's shared memory allow it; each CTA should own >= 64 Ki elements before it pays
 // for its per-tensor set-up and publishes.  Rejects tables whose shared memory exceeds the device's opt-in limit.
-template <class Op>
+template <class Op, class T>
 static int launch_multi_stream(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, const typename Op::Args &args, int op_param,
                                cudaStream_t st) {
     const size_t smem = ring_op_offset(count) + Op::smem_bytes(op_param);
@@ -625,17 +639,17 @@ static int launch_multi_stream(const ppq_b200_tensor_desc *descs, int count, int
         return (int)cudaGetLastError();
     if (smem > (size_t)limit) return (int)cudaErrorInvalidValue;
     // the > 48 KB opt-in is per device, not per process: set it on every launch
-    if (cudaFuncSetAttribute(multi_stream_kernel<Op>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    if (cudaFuncSetAttribute(multi_stream_kernel<Op, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
         return (int)cudaGetLastError();
     int resident = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, multi_stream_kernel<Op>, kRingThreads, smem) != cudaSuccess)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, multi_stream_kernel<Op, T>, kRingThreads, smem) != cudaSuccess)
         return (int)cudaGetLastError();
     if (resident < 1) resident = 1;
     if (resident > 2) resident = 2;
     int64_t g = ((int64_t)count * max_n + 65535) / 65536;
     if (g > (int64_t)sm_count() * resident) g = (int64_t)sm_count() * resident;
     if (g < 1) g = 1;
-    multi_stream_kernel<Op><<<(int)g, kRingThreads, smem, st>>>(descs, count, args);
+    multi_stream_kernel<Op, T><<<(int)g, kRingThreads, smem, st>>>(descs, count, args);
     return (int)cudaGetLastError();
 }
 
@@ -742,16 +756,30 @@ int ppq_b200_histogram_c(const float *x, int64_t n, int64_t epc, int C, float hi
     return (int)cudaGetLastError();
 }
 
+int ppq_b200_multi_minmax_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype, float *minmax_arena, void *stream) {
+    if (!valid_dtype(dtype) || count <= 0 || max_n <= 0 || !descs || !minmax_arena) return (int)cudaErrorInvalidValue;
+    return with_elem_type(dtype, [&](auto tag) {
+        return launch_multi_stream<MinMaxOp, decltype(tag)>(descs, count, max_n, MinMaxOp::Args{minmax_arena}, 0, (cudaStream_t)stream);
+    });
+}
+
 int ppq_b200_multi_minmax_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float *minmax_arena, void *stream) {
-    if (count <= 0 || max_n <= 0 || !descs || !minmax_arena) return (int)cudaErrorInvalidValue;
-    return launch_multi_stream<MinMaxOp>(descs, count, max_n, MinMaxOp::Args{minmax_arena}, 0, (cudaStream_t)stream);
+    return ppq_b200_multi_minmax_t_dt(descs, count, max_n, PPQ_B200_F32, minmax_arena, stream);
+}
+
+int ppq_b200_multi_histogram_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype, const float *hist_scale_arena,
+                                  int clip_outliers, int32_t *hist_arena, int64_t bins, void *stream) {
+    if (!valid_dtype(dtype) || count <= 0 || max_n <= 0 || !descs || !hist_scale_arena || !hist_arena || bins <= 0 || bins > kMaxSmemBins)
+        return (int)cudaErrorInvalidValue;
+    return with_elem_type(dtype, [&](auto tag) {
+        return launch_multi_stream<HistOp, decltype(tag)>(descs, count, max_n, HistOp::Args{hist_scale_arena, hist_arena, (int)bins, clip_outliers},
+                                                          (int)bins, (cudaStream_t)stream);
+    });
 }
 
 int ppq_b200_multi_histogram_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, const float *hist_scale_arena,
                                int clip_outliers, int32_t *hist_arena, int64_t bins, void *stream) {
-    if (count <= 0 || max_n <= 0 || !descs || !hist_scale_arena || !hist_arena || bins <= 0 || bins > kMaxSmemBins) return (int)cudaErrorInvalidValue;
-    return launch_multi_stream<HistOp>(descs, count, max_n, HistOp::Args{hist_scale_arena, hist_arena, (int)bins, clip_outliers}, (int)bins,
-                                       (cudaStream_t)stream);
+    return ppq_b200_multi_histogram_t_dt(descs, count, max_n, PPQ_B200_F32, hist_scale_arena, clip_outliers, hist_arena, bins, stream);
 }
 
 }  // extern "C"

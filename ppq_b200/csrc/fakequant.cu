@@ -605,6 +605,96 @@ ew_half_channel_kernel(const T *__restrict__ x, OutT *__restrict__ y, int64_t n,
     }
 }
 
+// ---- multi-tensor per-channel fake-quant of fp16 / bf16 weights: multi_channel_kernel's partition with 8-element vectors ----------------
+// Warp segments of 128 vectors (1024 elements), the concatenation of all segments split evenly over the CTAs.  A tensor whose x and y are
+// 16-byte aligned and whose rows are a multiple of 8 elements keeps every vector inside one channel row: one operator per segment when
+// the segment lies in one row, else one per vector (the rebuild rule of ew_half_channel_kernel).  Any other tensor (depth-wise 3x3
+// rows, unaligned views) is walked element by element.  y has the input's type: the fp32 result rounded once to nearest even.
+template <class Op, class T>
+__global__ void __launch_bounds__(kThreads)
+multi_channel_half_kernel(const ppq_b200_lc_desc *__restrict__ descs, int count, typename Op::Params p) {
+    extern __shared__ long long seg_prefix[];                          // [count + 1], in segments
+    constexpr int kSegElems = 8 * kSegVec;
+    for (int t = threadIdx.x; t < count; t += kThreads) {
+        const int64_t n = descs[t].n;
+        seg_prefix[t + 1] = n > 0 ? (n + kSegElems - 1) / kSegElems : 0;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        long long run = 0; seg_prefix[0] = 0;
+        for (int t = 1; t <= count; t++) { run += seg_prefix[t]; seg_prefix[t] = run; }
+    }
+    __syncthreads();
+    const int64_t total = seg_prefix[count];
+    const int64_t span = (total + gridDim.x - 1) / gridDim.x;
+    const int64_t s0 = (int64_t)blockIdx.x * span, s1 = (s0 + span) < total ? (s0 + span) : total;
+    if (s0 >= total) return;
+    int t;
+    { int lo = 0, hi = count - 1; while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (seg_prefix[mid] <= s0) lo = mid; else hi = mid - 1; } t = lo; }
+    const typename Op::Plan plan(p);
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (; t < count && seg_prefix[t] < s1; t++) {
+        const int64_t first = seg_prefix[t], segs = seg_prefix[t + 1] - first;
+        if (segs == 0) continue;
+        const ppq_b200_lc_desc d = descs[t];
+        const T *x = reinterpret_cast<const T *>(d.x);
+        T *y = reinterpret_cast<T *>(d.y);
+        const uint32_t a = (uint32_t)(s0 > first ? s0 - first : 0), b = (uint32_t)((s1 - first) < segs ? (s1 - first) : segs);
+        const bool al = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) == 0;
+        if (al && d.epc % 8 == 0) {
+            const uint4 *x8 = reinterpret_cast<const uint4 *>(x);
+            const uint32_t n8 = (uint32_t)(d.n >> 3), epc8 = (uint32_t)(d.epc >> 3);
+            const FastDiv32 de(epc8), dc((uint32_t)d.C);
+            // two 16-byte loads (16 elements) in flight per thread, two rounds per segment: four would not fit the registers without spilling
+            constexpr int kHalfUnroll = 2;
+            for (uint32_t sg = a + warp; sg < b; sg += kThreads / 32) {
+#pragma unroll 1
+                for (uint32_t base = sg * kSegVec; base < (sg + 1) * kSegVec; base += 32 * kHalfUnroll) {
+                    const uint32_t end = base + 32 * kHalfUnroll;
+                    uint4 v[kHalfUnroll];
+#pragma unroll
+                    for (int j = 0; j < kHalfUnroll; j++) if (base + j * 32 + lane < n8) v[j] = ld_stream_u4(x8 + base + j * 32 + lane);
+                    const uint32_t r0 = de.quot(base);
+                    const uint32_t c0 = r0 - dc.quot(r0) * (uint32_t)d.C;
+                    if ((r0 + 1) * epc8 >= end) {                        // the round lies inside one channel row (warp-uniform)
+                        const Op op(plan, __ldg(d.scale + c0), __ldg(d.offset + c0));
+#pragma unroll
+                        for (int j = 0; j < kHalfUnroll; j++) {
+                            const uint32_t vi = base + j * 32 + lane;
+                            if (vi < n8) { float4 lo, hi; unpack8<T>(v[j], lo, hi); EmitH<Op, T>::vec8(op, lo, hi, y, (int64_t)vi, true); }
+                        }
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < kHalfUnroll; j++) {
+                            const uint32_t vi = base + j * 32 + lane;
+                            if (vi < n8) {
+                                const uint32_t row = de.quot(vi);
+                                const uint32_t c = row - dc.quot(row) * (uint32_t)d.C;
+                                const Op op(plan, __ldg(d.scale + c), __ldg(d.offset + c));
+                                float4 lo, hi;
+                                unpack8<T>(v[j], lo, hi);
+                                EmitH<Op, T>::vec8(op, lo, hi, y, (int64_t)vi, true);
+                            }
+                        }
+                    }
+                }
+            }
+        } else {
+            const uint32_t n = (uint32_t)d.n;
+            const FastDiv32 de((uint32_t)d.epc), dc((uint32_t)d.C);
+            for (uint32_t sg = a + warp; sg < b; sg += kThreads / 32) {
+                const uint32_t e0 = sg * kSegElems, e1 = min(n, e0 + kSegElems);
+                for (uint32_t e = e0 + lane; e < e1; e += 32) {
+                    const uint32_t row = de.quot(e);
+                    const uint32_t c = row - dc.quot(row) * (uint32_t)d.C;
+                    const Op op(plan, __ldg(d.scale + c), __ldg(d.offset + c));
+                    EmitH<Op, T>::one(op, ld_stream1_f(x + e), y + e);
+                }
+            }
+        }
+    }
+}
+
 // ---- host-side launch helpers --------------------------------------------------------------------------------------------
 static inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -863,16 +953,32 @@ int ppq_b200_linear_quant_c_toint(const float *x, void *q, int out_bits, int64_t
     return ppq_b200_linear_quant_c_toint_dt(x, PPQ_B200_F32, q, out_bits, n, epc, C, scale, offset, qmin, qmax, rounding, stream);
 }
 
-int ppq_b200_multi_linear_quant_c(const ppq_b200_lc_desc *descs, int count, int64_t max_n, int qmin, int qmax, int rounding, void *stream) {
-    if (count <= 0 || count > kMaxMultiTensors || max_n <= 0 || max_n > 0x7fffffffLL || !descs || qmin > qmax) return (int)cudaErrorInvalidValue;
+int ppq_b200_multi_linear_quant_c_dt(const ppq_b200_lc_desc *descs, int count, int64_t max_n, int dtype, int qmin, int qmax, int rounding,
+                                     void *stream) {
+    if (!valid_dtype(dtype) || count <= 0 || count > kMaxMultiTensors || max_n <= 0 || max_n > 0x7fffffffLL || !descs || qmin > qmax) return (int)cudaErrorInvalidValue;
     // upper bound of the work (the true total is summed on the device): one CTA per 8 segments of 512 elements, at most 8 CTAs per SM
     int64_t g = ((int64_t)count * ((max_n + 4 * kSegVec - 1) / (4 * kSegVec)) + 7) / 8;
     if (g > (int64_t)sm_count() * 8) g = (int64_t)sm_count() * 8;
     const size_t smem = (size_t)(count + 1) * sizeof(long long);
+    if (dtype != PPQ_B200_F32) {                                       // the same bound in segments of 8 x kSegVec elements
+        g = ((int64_t)count * ((max_n + 8 * kSegVec - 1) / (8 * kSegVec)) + 7) / 8;
+        if (g > (int64_t)sm_count() * 8) g = (int64_t)sm_count() * 8;
+        return with_half_type(dtype, [&](auto tag) {
+            using T = decltype(tag);
+            if (rounding == RND_HALF_EVEN) multi_channel_half_kernel<LinearOp<0>, T><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, 0});
+            else if (rounding == RND_HALF_UP) multi_channel_half_kernel<LinearOp<RND_HALF_UP>, T><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, RND_HALF_UP});
+            else multi_channel_half_kernel<LinearOp<-1>, T><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, rounding});
+            return (int)cudaGetLastError();
+        });
+    }
     if (rounding == RND_HALF_EVEN) multi_channel_kernel<LinearOp<0>><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, 0});
     else if (rounding == RND_HALF_UP) multi_channel_kernel<LinearOp<RND_HALF_UP>><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, RND_HALF_UP});
     else multi_channel_kernel<LinearOp<-1>><<<(int)g, kThreads, smem, (cudaStream_t)stream>>>(descs, count, {qmin, qmax, rounding});
     return (int)cudaGetLastError();
+}
+
+int ppq_b200_multi_linear_quant_c(const ppq_b200_lc_desc *descs, int count, int64_t max_n, int qmin, int qmax, int rounding, void *stream) {
+    return ppq_b200_multi_linear_quant_c_dt(descs, count, max_n, PPQ_B200_F32, qmin, qmax, rounding, stream);
 }
 
 int ppq_b200_multi_linear_quant_t(const ppq_b200_lt_desc *descs, int count, int64_t max_n, int qmin, int qmax, int rounding, void *stream) {

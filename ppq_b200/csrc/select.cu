@@ -425,6 +425,11 @@ __device__ __forceinline__ bool select_pass(const T *__restrict__ x, int64_t a, 
 
 template <int TPB> __device__ __forceinline__ void finish_tensor_pass(SelectState *st, unsigned expected, bool *is_last);
 
+// passes 1-2 at six CTAs per SM (40 registers) for fp32; the half unpacking needs a few more registers (five CTAs per SM, no spill)
+template <class T> constexpr int kFilterCtas = std::is_same<T, float>::value ? 6 : 5;
+// span and piece boundaries of the table kernels fall on whole 16-byte vectors of the table's element type
+template <class T> constexpr int64_t kVecElems = 16 / sizeof(T);
+
 // Pass 0 with speculation (table form, `guess` given): the digit histogram of every element as in select_pass<0>, and on the way every key
 // beyond the thresholds remembered from the previous call of this slot (the previous batch of the same activation: the tail moves little
 // from batch to batch) is compacted -- except copies of the previously selected key, which are only counted.  When the candidates turn out
@@ -487,6 +492,7 @@ select_pass0_spec_kernel(const T *__restrict__ x, int64_t n, SelectState *__rest
     }
 }
 
+template <class T = float>
 __global__ void __launch_bounds__(kSelThreads, 1)
 multi_select_pass0_spec_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, SelectState *__restrict__ states,
                                uint32_t *__restrict__ bufs, int64_t cap) {
@@ -502,7 +508,7 @@ multi_select_pass0_spec_kernel(const ppq_b200_tensor_desc *__restrict__ descs, i
     __syncthreads();
     const int64_t total = prefix[count];
     int64_t span = (total + gridDim.x - 1) / gridDim.x;
-    span = (span + 3) & ~(int64_t)3;
+    span = (span + kVecElems<T> - 1) & ~(kVecElems<T> - 1);
     const int64_t s0 = (int64_t)blockIdx.x * span, s1 = (s0 + span) < total ? (s0 + span) : total;
     if (s0 >= total) return;
     int t = 0;
@@ -512,10 +518,10 @@ multi_select_pass0_spec_kernel(const ppq_b200_tensor_desc *__restrict__ descs, i
         if (d.n <= 0) continue;
         int64_t a = s0 - prefix[t]; if (a < 0) a = 0;
         int64_t b = s1 - prefix[t]; if (b > d.n) b = d.n;
-        a = (a + 3) & ~(int64_t)3; if (a > d.n) a = d.n;
-        if (b < d.n) b = (b + 3) & ~(int64_t)3; if (b > d.n) b = d.n;
+        a = (a + kVecElems<T> - 1) & ~(kVecElems<T> - 1); if (a > d.n) a = d.n;
+        if (b < d.n) b = (b + kVecElems<T> - 1) & ~(kVecElems<T> - 1); if (b > d.n) b = d.n;
         SelectState *st = states + t;
-        if (b > a) select_pass0_spec<kSelThreads>(d.x, a, b, threadIdx.x, kSelThreads, st, bufs + (int64_t)t * 2 * cap, cap, sh, sh_cnt);
+        if (b > a) select_pass0_spec<kSelThreads, T>(reinterpret_cast<const T *>(d.x), a, b, threadIdx.x, kSelThreads, st, bufs + (int64_t)t * 2 * cap, cap, sh, sh_cnt);
         const unsigned expected = (unsigned)((prefix[t + 1] - 1) / span - prefix[t] / span + 1);
         finish_tensor_pass<kSelThreads>(st, expected, &is_last);
         if (is_last) { __threadfence(); select_scan<0, kSelThreads>(st, cap); }
@@ -552,8 +558,13 @@ __device__ __forceinline__ void finish_tensor_pass(SelectState *st, unsigned exp
     __syncthreads();
 }
 
-template <int LEVEL, int TPB>
-__global__ void __launch_bounds__(TPB, LEVEL == 0 ? 2 : 6)
+// The table's element type T is one per launch (every descriptor's `x` points at elements of that type).  On top of the single-tensor
+// passes a table pass carries the span walk, so the half unpacking does not fit their register budgets without spilling: fp16 / bf16 run
+// pass 0 at one 1024-thread CTA per SM (64 registers, like the speculative pass 0) and passes 1-2 at four CTAs per SM.
+template <class T> constexpr int kTablePass0Ctas = std::is_same<T, float>::value ? 2 : 1;
+template <class T> constexpr int kTableFilterCtas = std::is_same<T, float>::value ? 6 : 4;
+template <int LEVEL, int TPB, class T = float>
+__global__ void __launch_bounds__(TPB, LEVEL == 0 ? kTablePass0Ctas<T> : kTableFilterCtas<T>)
 multi_select_pass_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int count, SelectState *__restrict__ states,
                          uint32_t *__restrict__ bufs, int64_t cap) {
     __shared__ int sh[2][kDigits];
@@ -568,7 +579,7 @@ multi_select_pass_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int cou
     __syncthreads();
     const int64_t total = prefix[count];
     int64_t span = (total + gridDim.x - 1) / gridDim.x;
-    span = (span + 3) & ~(int64_t)3;
+    span = (span + kVecElems<T> - 1) & ~(kVecElems<T> - 1);
     const int64_t s0 = (int64_t)blockIdx.x * span, s1 = (s0 + span) < total ? (s0 + span) : total;
     if (s0 >= total) return;
     int t = 0;
@@ -578,11 +589,11 @@ multi_select_pass_kernel(const ppq_b200_tensor_desc *__restrict__ descs, int cou
         if (d.n <= 0) continue;
         int64_t a = s0 - prefix[t]; if (a < 0) a = 0;
         int64_t b = s1 - prefix[t]; if (b > d.n) b = d.n;
-        a = (a + 3) & ~(int64_t)3; if (a > d.n) a = d.n;               // both neighbours round the shared boundary the same way
-        if (b < d.n) b = (b + 3) & ~(int64_t)3; if (b > d.n) b = d.n;
+        a = (a + kVecElems<T> - 1) & ~(kVecElems<T> - 1); if (a > d.n) a = d.n;   // both neighbours round the shared boundary the same way
+        if (b < d.n) b = (b + kVecElems<T> - 1) & ~(kVecElems<T> - 1); if (b > d.n) b = d.n;
         SelectState *st = states + t;
         bool active;                                                   // uniform over the grid
-        if (b > a) active = select_pass<LEVEL, TPB>(d.x, a, b, threadIdx.x, TPB, st, bufs + (int64_t)t * 2 * cap, cap, sh, sh_cnt);
+        if (b > a) active = select_pass<LEVEL, TPB, 4, (LEVEL != 0), T>(reinterpret_cast<const T *>(d.x), a, b, threadIdx.x, TPB, st, bufs + (int64_t)t * 2 * cap, cap, sh, sh_cnt);
         else active = level_needed<LEVEL>(st);                         // overlaps the tensor by less than a vector: no data, but a ticket
         if (active) {
             const unsigned expected = (unsigned)((prefix[t + 1] - 1) / span - prefix[t] / span + 1);
@@ -684,9 +695,6 @@ static inline int grid_filter(int64_t n) {
     return (int)(g < 1 ? 1 : g);
 }
 
-// passes 1-2 at six CTAs per SM (40 registers) for fp32; the half unpacking needs a few more registers (five CTAs per SM, no spill)
-template <class T> constexpr int kFilterCtas = std::is_same<T, float>::value ? 6 : 5;
-
 template <class T>
 static int select_two(const T *x, int64_t n, int q_mode, float q, long long r0, long long r1, float *out, void *workspace, cudaStream_t s,
                       uint32_t *guess = nullptr) {
@@ -775,9 +783,9 @@ int ppq_b200_quantile_t_guess(const float *x, int64_t n, float q, float *out2, v
     return ppq_b200_quantile_t_dt(x, PPQ_B200_F32, n, q, out2, workspace, guess, stream);
 }
 
-int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float q, float *out, int64_t out_stride,
-                              void *workspace, int64_t cap, uint32_t *guess, void *stream) {
-    if (count <= 0 || max_n <= 0 || !descs || !out || !workspace || cap <= 0 || out_stride < 2) return (int)cudaErrorInvalidValue;
+int ppq_b200_multi_quantile_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype, float q, float *out, int64_t out_stride,
+                                 void *workspace, int64_t cap, uint32_t *guess, void *stream) {
+    if (!valid_dtype(dtype) || count <= 0 || max_n <= 0 || !descs || !out || !workspace || cap <= 0 || out_stride < 2) return (int)cudaErrorInvalidValue;
     const size_t smem = (size_t)(count + 1) * sizeof(long long);
     if (smem > 24 * 1024) return (int)cudaErrorInvalidValue;
     cudaStream_t s = (cudaStream_t)stream;
@@ -786,14 +794,26 @@ int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int6
     int64_t work = (int64_t)count * max_n;
     int g0 = grid_pass0(work), g1 = grid_filter(work);
     select_init_kernel<<<count, 1024, 0, s>>>(states, descs, 0, q, 1, 0, 0, guess);
-    if (guess) {                                                        // 64 registers per thread: one 1024-thread CTA per SM
-        const int gs = g0 > sm_count() ? sm_count() : g0;
-        multi_select_pass0_spec_kernel<<<gs, kSelThreads, smem, s>>>(descs, count, states, bufs, cap);
-    } else multi_select_pass_kernel<0, kSelThreads><<<g0, kSelThreads, smem, s>>>(descs, count, states, bufs, cap);
-    multi_select_pass_kernel<1, kFilterThreads><<<g1, kFilterThreads, smem, s>>>(descs, count, states, bufs, cap);
-    multi_select_pass_kernel<2, kFilterThreads><<<g1 > 2 * sm_count() ? 2 * sm_count() : g1, kFilterThreads, smem, s>>>(descs, count, states, bufs, cap);
+    with_elem_type(dtype, [&](auto tag) {
+        using T = decltype(tag);
+        if (guess) {                                                    // 64 registers per thread: one 1024-thread CTA per SM
+            const int gs = g0 > sm_count() ? sm_count() : g0;
+            multi_select_pass0_spec_kernel<T><<<gs, kSelThreads, smem, s>>>(descs, count, states, bufs, cap);
+        } else {
+            const int resident = kTablePass0Ctas<T> * sm_count();
+            multi_select_pass_kernel<0, kSelThreads, T><<<g0 > resident ? resident : g0, kSelThreads, smem, s>>>(descs, count, states, bufs, cap);
+        }
+        multi_select_pass_kernel<1, kFilterThreads, T><<<g1, kFilterThreads, smem, s>>>(descs, count, states, bufs, cap);
+        multi_select_pass_kernel<2, kFilterThreads, T><<<g1 > 2 * sm_count() ? 2 * sm_count() : g1, kFilterThreads, smem, s>>>(descs, count, states, bufs, cap);
+        return 0;
+    });
     select_finish_kernel<<<2 * count, kSelThreads, 0, s>>>(states, bufs, cap, descs, out, out_stride, guess);
     return (int)cudaGetLastError();
+}
+
+int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float q, float *out, int64_t out_stride,
+                              void *workspace, int64_t cap, uint32_t *guess, void *stream) {
+    return ppq_b200_multi_quantile_t_dt(descs, count, max_n, PPQ_B200_F32, q, out, out_stride, workspace, cap, guess, stream);
 }
 
 int ppq_b200_isotone_t(const float *x, int64_t n, float *out4, void *workspace, void *stream) {

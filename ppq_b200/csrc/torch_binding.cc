@@ -344,6 +344,64 @@ void Multi_Quantile_T(const Tensor &descs, const int64_t max_numel, const float 
     CheckStatus(ppq_b200_multi_quantile_t(reinterpret_cast<const ppq_b200_tensor_desc *>(descs.data_ptr<int64_t>()), count, max_numel, q,
                                           out.data_ptr<float>(), out_stride, workspace.data_ptr(), cap, gp, Stream()), "Multi_Quantile_T");
 }
+// ---------------------------------------------------------------- fp16 / bf16 siblings of the table names
+// The positional signatures of the fp32 names with the table's element type after max_numel: a raw pointer table cannot tell it.
+int HalfTableType(const py::object &dtype) {
+    const auto st = torch::python::detail::py_object_to_dtype(dtype);
+    if (st == at::kHalf) return PPQ_B200_F16;
+    if (st == at::kBFloat16) return PPQ_B200_BF16;
+    throw KernelFailure("Kernel Failure, Invalid dtype of Input tensor: Value(Expect to be FP16 or BF16)");
+}
+void Multi_MinMax_T_Half(const Tensor &descs, const int64_t max_numel, const py::object &dtype, Tensor &minmax_arena) {
+    const int dt = HalfTableType(dtype);
+    CheckTensor(descs, at::kLong, "Descriptors(Expect to be INT64)");
+    CheckTensor(minmax_arena, at::kFloat, "MinMaxArena(Expect to be FP32)");
+    if (descs.dim() != 2 || descs.size(1) != 3 || !descs.is_contiguous()) throw KernelFailure("Kernel Failure, descriptor table must be [count, 3] int64.");
+    const c10::cuda::CUDAGuard guard(descs.device());
+    CheckStatus(ppq_b200_multi_minmax_t_dt(reinterpret_cast<const ppq_b200_tensor_desc *>(descs.data_ptr<int64_t>()), (int)descs.size(0),
+                                           max_numel, dt, minmax_arena.data_ptr<float>(), Stream()), "Multi_MinMax_T_Half");
+}
+void Multi_Histogram_T_Half(const Tensor &descs, const int64_t max_numel, const py::object &dtype, const Tensor &hist_scale_arena,
+                            const bool clip_outliers, Tensor &hist_arena, const int64_t bins) {
+    const int dt = HalfTableType(dtype);
+    CheckTensor(descs, at::kLong, "Descriptors(Expect to be INT64)");
+    CheckTensor(hist_scale_arena, at::kFloat, "HistScaleArena(Expect to be FP32)");
+    CheckTensor(hist_arena, at::kInt, "HistArena(Expect to be INT32)");
+    if (descs.dim() != 2 || descs.size(1) != 3 || !descs.is_contiguous()) throw KernelFailure("Kernel Failure, descriptor table must be [count, 3] int64.");
+    const c10::cuda::CUDAGuard guard(descs.device());
+    CheckStatus(ppq_b200_multi_histogram_t_dt(reinterpret_cast<const ppq_b200_tensor_desc *>(descs.data_ptr<int64_t>()), (int)descs.size(0),
+                                              max_numel, dt, F(hist_scale_arena), clip_outliers, hist_arena.data_ptr<int>(), bins, Stream()),
+                "Multi_Histogram_T_Half");
+}
+void Multi_Quantile_T_Half(const Tensor &descs, const int64_t max_numel, const py::object &dtype, const float q, Tensor &out,
+                           const int64_t out_stride, Tensor &workspace, const int64_t cap, const c10::optional<Tensor> &guess) {
+    const int dt = HalfTableType(dtype);
+    CheckTensor(descs, at::kLong, "Descriptors(Expect to be INT64)");
+    CheckTensor(out, at::kFloat, "Quantiles(Expect to be FP32)");
+    if (descs.dim() != 2 || descs.size(1) != 3 || !descs.is_contiguous()) throw KernelFailure("Kernel Failure, descriptor table must be [count, 3] int64.");
+    const int count = (int)descs.size(0);
+    if (workspace.scalar_type() != at::kByte || workspace.numel() < ppq_b200_multi_quantile_workspace_bytes(count, cap))
+        throw KernelFailure("Kernel Failure, quantile workspace is too small (see Multi_Quantile_Workspace_Bytes).");
+    const c10::cuda::CUDAGuard guard(descs.device());
+    uint32_t *gp = nullptr;
+    if (guess.has_value()) {
+        CheckTensor(*guess, at::kInt, "Guess(Expect to be INT32)");
+        if (!guess->is_contiguous() || guess->numel() % ppq_b200_quantile_guess_words() != 0) throw KernelFailure("Kernel Failure, quantile guess buffer has a wrong shape.");
+        gp = reinterpret_cast<uint32_t *>(guess->data_ptr<int>());
+    }
+    CheckStatus(ppq_b200_multi_quantile_t_dt(reinterpret_cast<const ppq_b200_tensor_desc *>(descs.data_ptr<int64_t>()), count, max_numel, dt, q,
+                                             out.data_ptr<float>(), out_stride, workspace.data_ptr(), cap, gp, Stream()), "Multi_Quantile_T_Half");
+}
+// descs as for Multi_QuantizeTensor_LC; x and y of every row point at elements of `dtype`
+void Multi_QuantizeTensor_LC_Half(const Tensor &descs, const int64_t max_numel, const py::object &dtype, const int clip_min, const int clip_max,
+                                  const int rounding) {
+    const int dt = HalfTableType(dtype);
+    CheckTensor(descs, at::kLong, "Descriptors(Expect to be INT64)");
+    if (descs.dim() != 2 || descs.size(1) != 7 || !descs.is_contiguous()) throw KernelFailure("Kernel Failure, descriptor table must be [count, 7] int64.");
+    const c10::cuda::CUDAGuard guard(descs.device());
+    CheckStatus(ppq_b200_multi_linear_quant_c_dt(reinterpret_cast<const ppq_b200_lc_desc *>(descs.data_ptr<int64_t>()), (int)descs.size(0), max_numel,
+                                                 dt, clip_min, clip_max, rounding, Stream()), "Multi_QuantizeTensor_LC_Half");
+}
 Tensor Quantile_Guess_Init(const int64_t slots, const Tensor &like) {
     const c10::cuda::CUDAGuard guard(like.device());
     Tensor g = at::empty({slots, ppq_b200_quantile_guess_words()}, like.options().dtype(at::kInt));
@@ -448,6 +506,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("Multi_MinMax_T", Multi_MinMax_T, "Multi_MinMax_T");
     m.def("Multi_Histogram_T", Multi_Histogram_T, "Multi_Histogram_T");
     m.def("Multi_Quantile_T", Multi_Quantile_T, "Multi_Quantile_T");
+    m.def("Multi_MinMax_T_Half", Multi_MinMax_T_Half, "Multi_MinMax_T_Half");
+    m.def("Multi_Histogram_T_Half", Multi_Histogram_T_Half, "Multi_Histogram_T_Half");
+    m.def("Multi_Quantile_T_Half", Multi_Quantile_T_Half, "Multi_Quantile_T_Half");
+    m.def("Multi_QuantizeTensor_LC_Half", Multi_QuantizeTensor_LC_Half, "Multi_QuantizeTensor_LC_Half");
     m.def("Quantile_Guess_Init", Quantile_Guess_Init, "Quantile_Guess_Init");
     m.def("Multi_Quantile_Workspace_Bytes", Multi_Quantile_Workspace_Bytes, "Multi_Quantile_Workspace_Bytes");
     m.def("MinMax_To_Scale_Offset", MinMax_To_Scale_Offset, "MinMax_To_Scale_Offset");

@@ -141,6 +141,7 @@ class TorchExecutor:
         self._names = {id(m): n for n, m in self.model.named_modules()}
         self._hooks, self._collect, self._collected, self._sink = None, False, None, None
         self._tracing, self._wq, self._swapped, self._bypass = True, {}, {}, False
+        self._mw = {}                                                    # weight dtype -> (signature, MultiWeightQuantizer, module ids)
         self._dequantized = None                                       # [(config, stored state)] while dequantize() is in effect
         self._produced = {}                                            # id(tensor) -> (operation, tensor, version at production)
         self._quant_fn = PPQuantFunction
@@ -213,31 +214,35 @@ class TorchExecutor:
 
     def _quantize_all_weights(self):
         """All activated per-channel linear weight configs that share (axis, range, rounding) are fake-quantised by ONE multi-tensor launch
-        at the start of the forward (the per-module results are what the pre-forward hooks hand to the operations).  Falls back to one
-        launch per weight for anything else (FP8 weights, mixed policies, fp16 / bf16 weights: the table kernel reads fp32 only)."""
-        from .calibration import MultiWeightQuantizer
+        at the start of the forward (the per-module results are what the pre-forward hooks hand to the operations) -- one table, and one
+        launch, per weight dtype present (fp32, fp16, bf16).  Falls back to one launch per weight for anything else (FP8 weights, mixed
+        policies)."""
+        from .calibration import TABLE_DTYPES, MultiWeightQuantizer
         from .core import QuantizationProperty as P
         ops = [self.operations[n] for n in self._order]
-        todo = [op for op in ops if op.weight_cfg is not None and QuantizationStates.is_activated(op.weight_cfg.state)
-                and op.weight_cfg.policy.has_property(P.LINEAR) and op.weight_cfg.policy.has_property(P.PER_CHANNEL)
-                and not op.weight_cfg.policy.has_property(P.DYNAMIC) and self._quant_fn is PPQuantFunction
-                and op.module.weight.dtype == torch.float32]
-        if len(todo) < 2: return {}
-        c0 = todo[0].weight_cfg
-        key0 = (c0.channel_axis, c0.quant_min, c0.quant_max, c0.rounding)
-        todo = [op for op in todo if (op.weight_cfg.channel_axis, op.weight_cfg.quant_min, op.weight_cfg.quant_max, op.weight_cfg.rounding) == key0]
-        sig = tuple((id(op.module), op.module.weight.data_ptr(), op.weight_cfg.scale.data_ptr(), op.weight_cfg.offset.data_ptr()) for op in todo)
-        if getattr(self, '_mw_sig', None) != sig:
-            dev = todo[0].module.weight.device
-            self._mw = MultiWeightQuantizer([op.module.weight.data for op in todo], [op.weight_cfg.scale.to(dev) for op in todo],
-                                            [op.weight_cfg.offset.to(dev) for op in todo], channel_axis=c0.channel_axis,
-                                            quant_min=c0.quant_min, quant_max=c0.quant_max,
-                                            rounding=c0.rounding.value if hasattr(c0.rounding, 'value') else int(c0.rounding))
-            # the quantizer keeps its own references to scale/offset: recompute the signature from what it actually points at
-            self._mw_sig = sig
-            self._mw_ids = [id(op.module) for op in todo]
-        outs = self._mw()
-        return dict(zip(self._mw_ids, outs))
+        tabled = [op for op in ops if op.weight_cfg is not None and QuantizationStates.is_activated(op.weight_cfg.state)
+                  and op.weight_cfg.policy.has_property(P.LINEAR) and op.weight_cfg.policy.has_property(P.PER_CHANNEL)
+                  and not op.weight_cfg.policy.has_property(P.DYNAMIC) and self._quant_fn is PPQuantFunction]
+        out = {}
+        for dtype in TABLE_DTYPES:
+            todo = [op for op in tabled if op.module.weight.dtype == dtype]
+            if len(todo) < 2: continue
+            c0 = todo[0].weight_cfg
+            key0 = (c0.channel_axis, c0.quant_min, c0.quant_max, c0.rounding)
+            todo = [op for op in todo if (op.weight_cfg.channel_axis, op.weight_cfg.quant_min, op.weight_cfg.quant_max, op.weight_cfg.rounding) == key0]
+            sig = tuple((id(op.module), op.module.weight.data_ptr(), op.weight_cfg.scale.data_ptr(), op.weight_cfg.offset.data_ptr()) for op in todo)
+            if self._mw.get(dtype, (None,))[0] != sig:
+                dev = todo[0].module.weight.device
+                mw = MultiWeightQuantizer([op.module.weight.data for op in todo], [op.weight_cfg.scale.to(dev) for op in todo],
+                                          [op.weight_cfg.offset.to(dev) for op in todo], channel_axis=c0.channel_axis,
+                                          quant_min=c0.quant_min, quant_max=c0.quant_max,
+                                          rounding=c0.rounding.value if hasattr(c0.rounding, 'value') else int(c0.rounding),
+                                          half_inputs=dtype != torch.float32)
+                # the quantizer keeps its own references to scale/offset: the signature is what it was built from
+                self._mw[dtype] = (sig, mw, [id(op.module) for op in todo])
+            _, mw, ids = self._mw[dtype]
+            out.update(zip(ids, mw()))
+        return out
 
     def _op_of(self, module, num_inputs: int = 1) -> QuantableOperation:
         idx = self._calls.get(id(module), 0)
@@ -552,7 +557,7 @@ def arena_settings(cfgs, method: str) -> dict:
 
 @torch.no_grad()
 def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=None, to_device=None, deferred='auto',
-                    graphs: bool = False, prefetch: bool = True, trace: list = None):
+                    graphs: bool = False, prefetch: bool = True, trace: list = None, half_inputs: bool = False):
     """Two-phase calibration of every observed activation through one ArenaCalibrator (statistics arena, one all-reduce per
     phase, on-device scale search).  `batches` is this rank's share of the calibration set (sample-sharded by the caller).
     deferred=False observes each tensor as the forward produces it (one launch per tensor);
@@ -566,19 +571,22 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     The observed configs must agree in range, bits, symmetry, power-of-two, minimum scale and bin / percentile overrides and be per-tensor
     (`arena_settings`); asymmetric 'kl' raises PermissionError as upstream, asymmetric 'mse' and more than 12287 KL bins raise ValueError --
     all before the first batch.
+    half_inputs=True calibrates fp16 / bf16 activations through the *_Half table kernels (scales and offsets are the fp32 ones on the upcasts): a
+    network cast to half, or an fp32 network when the caller wraps this call in torch.autocast -- its activations then arrive in both dtypes
+    and every deferred launch becomes one per dtype present.
     to_device: a callable applied to every batch, or 'ring' for host tensors staged through the device's persistent DeviceBatchRing.
     trace: a list that receives (phase, batch index, host time, CUDA event, thread CPU time) before every batch and at the end of a phase --
     bench.py's e2e uses it to say whether a slow calibration was slow on the host or on the device, and where."""
     import time
     half = sorted({str(p.dtype) for p in executor.model.parameters() if p.dtype != torch.float32})
-    if half:
+    if half and not half_inputs:
         raise TypeError(f'calibrate_arena: the multi-tensor collectors read fp32 tensors, this network has {", ".join(half)} parameters; '
                         'calibrate it with RuntimeCalibrationPass (per-observer collectors, which take fp16 / bf16).')
     from .calibration import ArenaCalibrator, is_dense
     cfgs = executor.observed_configs()
     if graphs and method == 'percentile': raise ValueError('graphs=True needs static statistics buffers; the percentile observer keeps one row per batch')
     dev = next(executor.model.parameters()).device
-    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group, **arena_settings(cfgs, method))
+    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group, half_inputs=half_inputs, **arena_settings(cfgs, method))
     for c in cfgs: c.observer_algorithm = method
     if iter(batches) is batches: batches = list(batches)                  # a one-shot iterator would leave phase 2 without data
     static_in = None
@@ -595,7 +603,7 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
             cal.begin_batch()
             if graphs:
                 if static_in is None:
-                    static_in = torch.empty(x.shape, dtype=torch.float32, device=dev)
+                    static_in = torch.empty(x.shape, dtype=x.dtype if half_inputs else torch.float32, device=dev)
                 static_in.copy_(x, non_blocking=True)
                 if graph is None:
                     # eager run on a side stream first (cuDNN autotuning, lazy initialisation), statistics restored afterwards:
