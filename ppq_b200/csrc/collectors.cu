@@ -174,8 +174,9 @@ struct SymBin {
     __device__ __forceinline__ SymBin(float hist_scale, int nbins, bool clip_outliers) : bins(nbins), last(nbins - 1), clip(clip_outliers) { d.init(hist_scale); }
     __device__ __forceinline__ explicit SymBin(const BinParams &p) : SymBin(p.a, p.bins, p.clip != 0) {}
     __device__ __forceinline__ unsigned finish(float t) const {
-        const int b = __float2int_rd(t);                              // (int) floor(.), saturating, NaN -> 0; never negative here
-        return clip ? min((unsigned)b, bins) : (unsigned)min(b, last);
+        const int b = __float2int_rd(t);                              // (int) floor(.), saturating, NaN -> 0
+        // negative only for a negative (or -0.0) hist_scale: dropped under clip (wraps above `bins` -> trash), else bin 0, as AsymBin
+        return clip ? min((unsigned)b, bins) : (unsigned)max(min(b, last), 0);
     }
     __device__ __forceinline__ unsigned operator()(float v) const { return finish(d.div(fabsf(v))); }
     __device__ __forceinline__ uint4 bin4(const float4 &v) const {
