@@ -240,6 +240,33 @@ PPQ_B200_API int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, in
 PPQ_B200_API int ppq_b200_multi_quantile_t_dt(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, int dtype, float q,
                                               float *out, int64_t out_stride, void *workspace, int64_t cap, uint32_t *guess, void *stream);
 
+/* ---- quantisation error analysis ----------------------------------------------------------------------------- */
+/* One (prediction, reference) pair of a paired-moment table: `rows` sample rows of `row_len` elements each, contiguous one after the other
+ * from `pred` and from `real` (a sample is the outermost dimension, or the whole tensor of a 1-d pair: ppq/quantization/measure/norm.py:36-38).
+ * Row i of the pair writes out row out_row0 + i.  Lives in DEVICE memory; pred and real may alias. */
+typedef struct {
+    const void *pred;      /* elements of the table's type */
+    const void *real;
+    int64_t     rows;
+    int64_t     row_len;
+    int64_t     out_row0;
+} ppq_b200_pair_desc;
+/* For every row of every pair, out[row] = {sum (p - r)^2, sum r^2, sum p^2, sum p * r} in fp64 (out: DEVICE double[total_rows][4], 16-byte
+ * aligned, rows no pair covers are left as they are; the row ranges of the pairs must not overlap).  The products are exact in fp64 and the
+ * only roundings are the additions (sum (p - r)^2 also rounds p - r when the exponents of p and r are more than 29 apart); the result is
+ * bit-identical from run to run and under CUDA-graph replay.  The longest chain of additions a term goes through is 74 + ceil(row_len / 16384).
+ * NaN and +-inf propagate as IEEE fp64 arithmetic gives them.  Every byte is read once.
+ * total_elems >= the sum of rows * row_len over the table; `workspace`: DEVICE scratch of
+ * ppq_b200_multi_paired_moments_workspace_bytes(total_rows, total_elems) bytes, 16-byte aligned.  count <= 2048; count == 0 or
+ * total_rows == 0 writes nothing.  A table the arguments do not describe (negative fields, an out row range outside [0, total_rows), more
+ * elements than total_elems) writes NaN into all total_rows rows. */
+PPQ_B200_API int64_t ppq_b200_multi_paired_moments_workspace_bytes(int64_t total_rows, int64_t total_elems);
+PPQ_B200_API int ppq_b200_multi_paired_moments(const ppq_b200_pair_desc *descs, int count, int64_t total_rows, int64_t total_elems,
+                                               double *out, void *workspace, void *stream);
+/* the same for a table whose pairs all have element type `dtype` (p and r alike): the moments of the exact upcasts. */
+PPQ_B200_API int ppq_b200_multi_paired_moments_dt(const ppq_b200_pair_desc *descs, int count, int64_t total_rows, int64_t total_elems,
+                                                  int dtype, double *out, void *workspace, void *stream);
+
 /* ---- scale / offset search on the device ---------------------------------------------------------------------- */
 /* replaces minmax_to_scale_offset, ppq/quantization/observer/range.py:22-75, vectorised over `count` ranges
  * (tensors or channels); arithmetic in fp64 like the Python original, results stored as fp32. */

@@ -29,7 +29,7 @@ NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-fmad=false',
               '--expt-relaxed-constexpr', '--expt-extended-lambda',
               '-Xcompiler', '-fPIC,-fvisibility=hidden,-ffp-contract=off,-Wall', '-I', INCLUDE]
-CU_SOURCES = ['fakequant.cu', 'fakequant_tma.cu', 'collectors.cu', 'search.cu', 'select.cu', 'train.cu', 'host.cc']
+CU_SOURCES = ['fakequant.cu', 'fakequant_tma.cu', 'collectors.cu', 'search.cu', 'select.cu', 'train.cu', 'analyse.cu', 'host.cc']
 HEADERS = ['common.cuh', 'ops.cuh', 'half.cuh', 'variants.h', os.path.join(INCLUDE, 'ppq_b200.h')]
 
 

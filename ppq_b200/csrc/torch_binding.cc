@@ -471,6 +471,31 @@ std::vector<Tensor> MSE_Search(const Tensor &hist_arena, const int64_t bins, con
                                     min_scale, interval, scale.data_ptr<float>(), offset.data_ptr<float>(), Stream()), "MSE_Search");
     return {scale, offset};
 }
+// descs: int64 tensor [count, 5] on the device = (pred, real, rows, row_len, out_row0) -- bit-compatible with ppq_b200_pair_desc; every pair
+// of the table has element type `dtype` (fp32, fp16 or bf16).  out: fp64 [total_rows, 4]; workspace: uint8 of at least
+// Multi_Paired_Moments_Workspace_Bytes(total_rows, total_elems) bytes.  An empty table writes nothing.
+void Multi_Paired_Moments(const Tensor &descs, const int64_t total_elems, const py::object &dtype, Tensor &out, Tensor &workspace) {
+    const auto st = torch::python::detail::py_object_to_dtype(dtype);
+    const int dt = st == at::kFloat ? PPQ_B200_F32 : HalfTableType(dtype);
+    if (descs.scalar_type() != at::kLong || descs.dim() != 2 || descs.size(1) != 5 || !descs.is_contiguous())
+        throw KernelFailure("Kernel Failure, descriptor table must be [count, 5] int64.");
+    if (out.scalar_type() != at::kDouble || out.dim() != 2 || out.size(1) != 4 || !out.is_contiguous())
+        throw KernelFailure("Kernel Failure, moments must be a contiguous [rows, 4] fp64 tensor.");
+    if (workspace.scalar_type() != at::kByte || !workspace.is_contiguous())
+        throw KernelFailure("Kernel Failure, paired-moment workspace must be a contiguous uint8 tensor.");
+    if (descs.size(0) == 0) return;
+    if (!descs.is_cuda() || !out.is_cuda() || !workspace.is_cuda() || descs.device() != out.device() || workspace.device() != out.device())
+        throw KernelFailure("Kernel Failure, descriptors, moments and workspace must be on one CUDA device.");
+    if (workspace.numel() < ppq_b200_multi_paired_moments_workspace_bytes(out.size(0), total_elems))
+        throw KernelFailure("Kernel Failure, paired-moment workspace is too small (see Multi_Paired_Moments_Workspace_Bytes).");
+    const c10::cuda::CUDAGuard guard(out.device());
+    CheckStatus(ppq_b200_multi_paired_moments_dt(reinterpret_cast<const ppq_b200_pair_desc *>(descs.data_ptr<int64_t>()), (int)descs.size(0),
+                                                 out.size(0), total_elems, dt, out.data_ptr<double>(), workspace.data_ptr(), Stream()),
+                "Multi_Paired_Moments");
+}
+int64_t Multi_Paired_Moments_Workspace_Bytes(const int64_t total_rows, const int64_t total_elems) {
+    return ppq_b200_multi_paired_moments_workspace_bytes(total_rows, total_elems);
+}
 int set_variant(const std::string &kernel, int variant) { return ppq_b200_set_variant(kernel.c_str(), variant); }
 int get_variant(const std::string &kernel) { return ppq_b200_get_variant(kernel.c_str()); }
 
@@ -516,6 +541,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("Hist_Scale_From_MinMax", Hist_Scale_From_MinMax, "Hist_Scale_From_MinMax");
     m.def("KL_Search", KL_Search, "KL_Search");
     m.def("MSE_Search", MSE_Search, "MSE_Search");
+    m.def("Multi_Paired_Moments", Multi_Paired_Moments, "Multi_Paired_Moments");
+    m.def("Multi_Paired_Moments_Workspace_Bytes", Multi_Paired_Moments_Workspace_Bytes, "Multi_Paired_Moments_Workspace_Bytes");
     m.def("set_variant", set_variant, "set_variant");
     m.def("get_variant", get_variant, "get_variant");
     m.def("abi_version", ppq_b200_abi_version, "abi_version");

@@ -143,6 +143,7 @@ class TorchExecutor:
         self._tracing, self._wq, self._swapped, self._bypass = True, {}, {}, False
         self._mw = {}                                                    # weight dtype -> (signature, MultiWeightQuantizer, module ids)
         self._dequantized = None                                       # [(config, stored state)] while dequantize() is in effect
+        self._only = None                                              # the operation quantize_only() runs quantised
         self._produced = {}                                            # id(tensor) -> (operation, tensor, version at production)
         self._quant_fn = PPQuantFunction
         for m in self.model.modules():
@@ -444,6 +445,29 @@ class TorchExecutor:
         self._dequantized = None
         return self
 
+    def quantize_only(self, name: Optional[str]):
+        """While dequantize() is in effect: operation `name` alone runs quantised -- its configs get their stored states back and its baked
+        weight is swapped in (QuantableOperation.restore_quantize_state of that one operation, IR/quantize.py:143-160), every other config stays
+        FP32.  quantize_only(None) returns that operation to FP32, and must precede restore_quantize_state()."""
+        if self._dequantized is None: raise RuntimeError('quantize_only: call dequantize() first')
+        self._restore_weights()
+        if self._only is not None:
+            op = self.operations[self._only]
+            for cfg in self._configs_of(op): cfg.state = QuantizationStates.FP32
+            if op.stored_weight is not None: op.module.weight.data, op.stored_weight = op.stored_weight, op.module.weight.data
+            self._only = None
+        if name is not None:
+            op = self.operations[name]
+            stored = {id(cfg): state for cfg, state in self._dequantized}
+            for cfg in self._configs_of(op): cfg.state = stored[id(cfg)]
+            if op.stored_weight is not None: op.module.weight.data, op.stored_weight = op.stored_weight, op.module.weight.data
+            self._only = name
+        return self
+
+    @staticmethod
+    def _configs_of(op: QuantableOperation) -> List[TensorQuantizationConfig]:
+        return op.input_cfgs + ([op.weight_cfg] if op.weight_cfg is not None else []) + [op.output_cfg]
+
 
 def _min_scale_of(cfg) -> float:
     from .core import OBSERVER_MIN_SCALE, OBSERVER_MIN_SCALE_MANUL_OVERRIDE
@@ -738,6 +762,81 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
     vals = (acc_t / count).tolist()
     del acc
     return dict(zip(names, vals))
+
+
+@torch.no_grad()
+def layerwise_error_analyse(executor: TorchExecutor, batches, interested_outputs=None, method: str = 'snr', steps: int = 8,
+                            to_device=None) -> Dict[str, float]:
+    """Which operation causes the quantisation error (ppq/quantization/analyse/layerwise.py:15-134): for every computing operation (Conv, Gemm,
+    ConvTranspose, MatMul, in executor order), the error of the interested outputs when that operation alone is quantised -- its configs with
+    their stored states and its baked weight, every other config FP32 (TorchExecutor.quantize_only) -- against the fp32 network.
+    Returns {operation name: measure}, measure = 'snr' (noise / signal power), 'mse' or 'cosine' per sample, averaged over the samples of a
+    batch and then over the updates as the reference's MeasureRecorder(reduce='mean') does: one update per (batch, interested output) weighted
+    by the output's shape[0], running mean (m n + r b) / (n + b) in Python doubles, batch by batch.
+    interested_outputs: None = the network's return value (a tensor, or every tensor of a tuple / list, in order); a name or a list of
+    operation names = those operations' outputs as the executor hands them on.  steps: the reference breaks after the update of batch
+    `steps`, so min(len(batches), steps + 1) batches are measured.
+    The loop is batch-outer: one fp32 forward per batch, kept on the device and measured against each operation's quantised forward of that
+    batch, (K + 1)(S + 1) forwards instead of the reference's 2 K (S + 1); the result is the reference's whenever the forward is deterministic
+    (deterministic cuDNN).  Each quantised forward's outputs go to one Multi_Paired_Moments launch; the per-sample measures and batch means
+    are fp64 on the device, and one copy to the host at the end feeds the running means.  The measure is the value in exact arithmetic
+    rounded once per fp64 addition, where the reference sums in fp32 (fp16 / bf16 outputs: their exact upcasts) -- DESIGN.md §2.
+    Every config's state, scale and offset and every weight are as before the call, also when a batch raises."""
+    import itertools
+
+    from .measure import MEASURES, batch_measures
+    if method not in MEASURES: raise ValueError(f"Unsupported measurement {method!r}: 'snr', 'mse' and 'cosine' are supported")
+    names = [n for n, op in executor.quantable_operations() if op.kind in COMPUTING_OP]
+    if isinstance(interested_outputs, str): interested_outputs = [interested_outputs]
+    if interested_outputs is not None:
+        unknown = [n for n in interested_outputs if n not in executor.operations]
+        if unknown: raise KeyError(f'layerwise_error_analyse: no operation named {", ".join(unknown)}')
+
+    class Tap:
+        def __init__(self, store): self.store = store
+        def pre_forward_hook(self, **kw): pass
+        def post_forward_hook(self, outputs, quant_outputs, quant_configs): self.store.append(quant_outputs[0].clone())
+
+    def run(x) -> List[torch.Tensor]:
+        if interested_outputs is None:
+            out = executor.forward(x)
+            outs = list(out) if isinstance(out, (tuple, list)) else [out]
+            if not all(isinstance(t, torch.Tensor) for t in outs): raise TypeError('layerwise_error_analyse: the network must return tensors')
+            return outs
+        taps = {n: [] for n in interested_outputs}
+        executor.forward(x, hooks={n: Tap(taps[n]) for n in interested_outputs})
+        return [taps[n][-1] for n in interested_outputs]
+
+    dev = next(executor.model.parameters()).device
+    res, weights = [], []                                                 # per batch: [K, outputs] fp64 on the device
+    executor.dequantize()
+    try:
+        for x in itertools.islice(batches, steps + 1):                   # read once: a one-shot iterator is enough
+            if to_device is not None: x = x.to(dev, non_blocking=True) if isinstance(to_device, str) else to_device(x)
+            real = run(x)
+            res.append(torch.empty(len(names), len(real), dtype=torch.float64, device=dev))
+            weights.append([int(t.shape[0]) for t in real])
+            for k, n in enumerate(names):
+                executor.quantize_only(n)
+                pred = run(x)
+                executor.quantize_only(None)
+                batch_measures(pred, real, method, out=res[-1][k])
+            del real
+    finally:
+        if executor._dequantized is not None: executor.quantize_only(None)
+        executor.restore_quantize_state()
+    results = {n: 0.0 for n in names}
+    if not weights: return results
+    vals = torch.stack(res).cpu().tolist()                                # [batches, K, outputs]
+    for k, n in enumerate(names):                                         # MeasureRecorder.update (analyse/util/__init__.py:32-47)
+        m, cnt = 0.0, 0
+        for b, ws in enumerate(weights):
+            for j, e in enumerate(ws):
+                m = m * cnt + vals[b][k][j] * e
+                cnt += e
+                m /= cnt
+        results[n] = m
+    return results
 
 
 def e2e_calibration_benchmark(batch: int, batches: int, steps: int, warmup: int, device, world: int = 1, seed: int = 0, graphs: bool = False,
