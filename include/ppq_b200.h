@@ -233,6 +233,8 @@ PPQ_B200_API int ppq_b200_multi_histogram_t_dt(const ppq_b200_tensor_desc *descs
  * the exact order statistics.  An entry with n = 0 has no order statistics: its two output values and its guess words are left as they are. */
 PPQ_B200_API int64_t ppq_b200_multi_quantile_workspace_bytes(int count, int64_t cap);
 PPQ_B200_API int64_t ppq_b200_quantile_guess_words(void);
+/* One 32-byte host-to-device copy per slot, enqueued on `stream` from a static host row: it does not wait for the stream and can be
+ * captured into a CUDA graph (tests/test_gpu_stream_contract.py, Quantile_Guess_Init). */
 PPQ_B200_API int ppq_b200_quantile_guess_init(uint32_t *guess, int64_t slots, void *stream);
 PPQ_B200_API int ppq_b200_multi_quantile_t(const ppq_b200_tensor_desc *descs, int count, int64_t max_n, float q,
                                            float *out, int64_t out_stride, void *workspace, int64_t cap, uint32_t *guess, void *stream);
