@@ -77,12 +77,17 @@ __device__ __forceinline__ float key_to_float(uint32_t k) {
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
 }
 
-// index arithmetic of _Quantile_T (sort.cu:13-19): int64 * float -> float, __float2int_rn (half-even, saturating), CLIP<int>(pos, 0, n - 1)
-__device__ __forceinline__ long long quantile_rank(int64_t n, float frac) {
-    int pos = __float2int_rn((float)n * frac);
-    const int last = (int)(n - 1);
-    pos = pos > last ? last : pos;
-    return pos < 0 ? 0 : pos;
+// index arithmetic of _Quantile_T (sort.cu:13-19) in 64 bits: int64 * float -> float, round half-even, clip to [0, n - 1] (NaN -> 0).
+// For n <= 2^31 this is the reference's __float2int_rn + CLIP<int> exactly (n - 1 fits an int, so the int saturation never decides);
+// above, the reference's `(int)(n - 1)` goes negative and it reads out of bounds, while this keeps the rank the formula gives (DESIGN §2).
+// One definition for the init kernel and the host's sampling decision in select_two.
+__host__ __device__ inline long long quantile_rank(int64_t n, float frac) {
+    const float f = (float)n * frac;
+    if (!(f > 0.0f)) return 0;
+    const float r = rintf(f);                                          // half-even (the default rounding mode on the host)
+    if (r >= 9223372036854775808.0f) return n - 1;
+    const long long pos = (long long)r;
+    return pos > n - 1 ? n - 1 : pos;
 }
 
 // Block-wide search of the bucket that contains rank k in a 2048-bin histogram (TPB threads, kDigits / TPB consecutive bins per thread, warp
@@ -223,8 +228,10 @@ __device__ __noinline__ void select_scan(SelectState *st, long long cap) {
             for (int r = 0; r < 2; r++) {
                 const long long app = (long long)__ldcg(&st->ccount[r]), eq = (long long)__ldcg(&st->eqc[r]), cnt = app + eq;
                 const long long need = r == 0 ? n - st->rank[0] : st->rank[1] + 1;
+                // the 32-bit copy count is exact while the top-digit bucket of k[r] (64-bit histogram) holds fewer than 2^32 elements
+                const bool eq_exact = __ldcg(&st->hist[0][st->k[r] >> 21]) <= 0xFFFFFFFFull;
                 unsigned int d = st->d[r];
-                if (app <= cap && cnt >= need) {
+                if (app <= cap && cnt >= need && eq_exact) {
                     st->mode[r] = kModeCompact; st->compacted[r] = 1u; st->clevel[r] = 0u; st->prefix[r] = 0u; st->cbuf[r] = (unsigned)r;
                     st->rank[r] = r == 0 ? cnt - need : st->rank[1];
                     st->veq[r] = (unsigned)eq; st->vkey[r] = st->k[r];
@@ -233,7 +240,8 @@ __device__ __noinline__ void select_scan(SelectState *st, long long cap) {
                     st->ccount[r] = 0u;                                              // the buffer goes back to the regular compaction of pass 1
                     const bool first_call = r == 0 ? st->g[0] == 0xFFFFFFFFu : st->g[1] == 0u;   // nothing was guessed yet: no verdict on the margin
                     if (app > cap) { if (d > kSpecMarginMin) d >>= 1; }
-                    else if (!first_call && d < kSpecMarginMax) d <<= 1;             // too few candidates: the distribution moved, widen
+                    else if (eq_exact && !first_call && d < kSpecMarginMax) d <<= 1; // too few candidates: the distribution moved, widen
+                    // (a copy count too large to trust says nothing about the margin: it stays)
                 }
                 st->d[r] = d;
             }
@@ -445,10 +453,13 @@ __device__ __forceinline__ void select_pass0_spec(const T *__restrict__ x, int64
     const uint32_t a0 = (uint32_t)__cvta_generic_to_shared(&sh[0][0]);
     uint32_t *buf[2] = {bufs, bufs + cap};
     unsigned eq_hi = 0, eq_lo = 0;
+    // A thread that has seen the buffer full stops reserving: the verdict is already "too many candidates", and the 32-bit count stays
+    // below cap + one reservation per thread + one flush per CTA instead of wrapping on a tensor of 2^32 candidates.
+    bool full[2] = {false, false};
     auto append = [&](int r, uint32_t k) {
         const unsigned idx = atomicAdd(&sh_cnt[r], 1u);
         if (idx < (unsigned)kHalf) sh[1][r * kHalf + idx] = (int)k;
-        else { const unsigned gi = atomicAdd(&st->ccount[r], 1u); if ((long long)gi < cap) buf[r][gi] = k; }
+        else if (!full[r]) { const unsigned gi = atomicAdd(&st->ccount[r], 1u); if ((long long)gi < cap) buf[r][gi] = k; else full[r] = true; }
     };
     auto candidate = [&](uint32_t k) {
         if (k >= g_hi) { if (k == k_hi) eq_hi++; else append(0, k); }
@@ -638,7 +649,7 @@ select_finish_kernel(const SelectState *__restrict__ states, const uint32_t *__r
             }
         }
         const uint32_t vkey = st->vkey[r];
-        const unsigned veq = st->veq[r];
+        const unsigned long long veq = st->veq[r];                                              // up to 2^32 - 1: added in 64 bits
         for (int level = (int)st->clevel[r]; level <= 2; level++) {
             const int shift = level_shift(level);
             const uint32_t dmask = level_dmask(level), pmask = level_pmask(level), want = key & pmask;
@@ -664,10 +675,9 @@ select_finish_kernel(const SelectState *__restrict__ states, const uint32_t *__r
                     if (i < m && (v[j] & pmask) == want) atomicAdd(&sh[(v[j] >> shift) & dmask], 1);
                 }
             }
-            if (threadIdx.x == 0 && veq && (vkey & pmask) == want)                            // the counted-only copies of the threshold key
-                atomicAdd(&sh[(vkey >> shift) & dmask], (int)veq);
+            const int vd = (veq && (vkey & pmask) == want) ? (int)((vkey >> shift) & dmask) : -1;   // the counted-only copies of the threshold key
             __syncthreads();
-            block_pick<kSelThreads>([&](int i) { return (unsigned long long)sh[i]; }, k, &s_digit, &s_before, &s_cnt);
+            block_pick<kSelThreads>([&](int i) { return (unsigned long long)sh[i] + (i == vd ? veq : 0ull); }, k, &s_digit, &s_before, &s_cnt);
             key |= s_digit << shift;
             k -= s_before;
             __syncthreads();
@@ -704,8 +714,7 @@ static int select_two(const T *x, int64_t n, int q_mode, float q, long long r0, 
     // cold call on a big tensor: thresholds from a sample (select_init_kernel), unless both tails are too heavy for the compaction buffer
     bool sample = false;
     if (q_mode && n >= kSampleMinElems && !(variant_of(kVarSelect) & 64)) {
-        auto rank_of = [&](float frac) { long long pos = (long long)nearbyintf((float)n * frac); pos = pos > n - 1 ? n - 1 : pos; return pos < 0 ? 0 : pos; };
-        const long long need_hi = n - rank_of(q), need_lo = rank_of(1.0f - q) + 1;
+        const long long need_hi = n - quantile_rank(n, q), need_lo = quantile_rank(n, 1.0f - q) + 1;
         sample = sample_rank_ok(sample_rank_from_end(need_hi, n), n, cap) || sample_rank_ok(sample_rank_from_end(need_lo, n), n, cap);
     }
     uint32_t *sample_keys = bufs + 2 * cap;
