@@ -682,9 +682,50 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     return cal
 
 
+def _analysis_world(group) -> int:
+    """How many ranks share an analysis: the size of `group`, or 1 for group=None (torch.distributed is not touched then, so a caller may run
+    the analysis on one rank of an initialised job)."""
+    if group is None: return 1
+    import torch.distributed as dist
+    return dist.get_world_size(group)
+
+
+def _my_batches(batches, limit: Optional[int], group, fn: str):
+    """This rank's share of global batches 0 .. n-1, n = len(batches) cut to `limit` (r, r + R, ...: calibration.shard_indices), read from
+    `batches` by index one at a time."""
+    import torch.distributed as dist
+
+    from .calibration import shard_indices
+    if not (hasattr(batches, '__len__') and hasattr(batches, '__getitem__')):
+        raise TypeError(f'{fn}: a sharded analysis indexes its batches; pass a sequence that is the same on every rank, '
+                        f'not {type(batches).__name__}')
+    n = len(batches) if limit is None else min(len(batches), limit)
+    return (batches[i] for i in shard_indices(n, dist.get_rank(group), dist.get_world_size(group)))
+
+
+def _gather_in_batch_order(blocks: List[torch.Tensor], rows: int, dtype: torch.dtype, failed: Optional[BaseException], group,
+                           fn: str) -> Optional[torch.Tensor]:
+    """The one exchange of a sharded analysis.  blocks: this rank's per-batch [rows, width] results in its batch order.  First an
+    all_reduce(MIN) of {ok, -width}: a rank whose batch raised makes every rank raise (the failing rank its own error) instead of leaving the
+    others waiting in the gather, and a rank without a batch learns the width.  Then every rank's blocks are all-gathered and put in global
+    batch order: [rows, n, width] (CUDA tensors for NCCL, host tensors otherwise), or None when no rank had a batch."""
+    import torch.distributed as dist
+
+    from .calibration import gather_in_sample_order
+    dev = torch.device('cuda', torch.cuda.current_device()) if dist.get_backend(group) == 'nccl' else torch.device('cpu')
+    status = torch.tensor([0 if failed is not None else 1, -(blocks[0].shape[1] if blocks else 0)], dtype=torch.int64, device=dev)
+    dist.all_reduce(status, op=dist.ReduceOp.MIN, group=group)
+    ok, width = status.tolist()
+    if failed is not None: raise failed
+    if not ok: raise RuntimeError(f'{fn}: a batch raised on another rank')
+    if width == 0: return None
+    local = torch.stack(blocks, dim=1).to(dev) if blocks else torch.zeros(rows, 0, -width, dtype=dtype, device=dev)
+    return gather_in_sample_order(local, group)
+
+
 @torch.no_grad()
 def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, graphs: bool = False, fetchs: Optional[int] = None,
-                            seed: int = 10086) -> Dict[str, float]:
+                            seed: int = 10086, group=None) -> Dict[str, float]:
     """The evaluation loop where fake-quant throughput shows up in user wall-clock (ppq/quantization/analyse/graphwise.py:64-183): run every batch
     through the network twice -- all configs dequantised (fp32) and all configs active -- and report, per quantable operation, the SNR
     mean((q - f)^2) / mean(f^2) per sample, averaged (torch_snr_error, ppq/quantization/measure/norm.py:52-93).  Every activation goes through
@@ -694,7 +735,14 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
     (python -> binding -> allocator -> launch, 4.5-5 us x every config x every forward) disappears from the loop.
     fetchs=None measures on whole tensors, every quantable operation.  fetchs=4096 follows the reference to the letter: computing operations
     only (graphwise.py:112-113), `fetchs` elements per sample picked by the reference's seeded linear congruential indexer
-    (utils/fetch.py:4-23, seed 10086) -- pinned against the real function on the GPU (tests/test_gpu_graph_parity.py)."""
+    (utils/fetch.py:4-23, seed 10086) -- pinned against the real function on the GPU (tests/test_gpu_graph_parity.py).
+    group: a torch.distributed process group of R > 1 ranks shards the batches -- `batches` is a sequence, the same on every rank, and rank r
+    runs global batches r, r + R, ... of it; the per-batch SNR vectors are gathered in global batch order and summed in that order, so every
+    rank returns the single-process report (bit for bit with a deterministic forward on one GPU model: DESIGN.md §6).  A batch that raises on
+    one rank makes every rank raise.  group=None runs every batch here and never calls torch.distributed."""
+    fn = 'graphwise_error_analyse'
+    world = _analysis_world(group)
+    if world > 1: batches = _my_batches(batches, None, group, fn)
     names = [n for n, op in executor.quantable_operations() if fetchs is None or op.kind in COMPUTING_OP]
     acc = {n: None for n in names}
     count = 0
@@ -728,6 +776,7 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
         return torch.stack(out)
 
     static_in, graph, fp, qt, static_snr = None, None, {}, {}, None
+    mine, failed = [], None                                               # sharded: this rank's per-batch [K, 1] SNR, its error
     try:
         for x in batches:
             if to_device is not None: x = x.to(next(executor.model.parameters()).device, non_blocking=True) if isinstance(to_device, str) else to_device(x)
@@ -754,10 +803,22 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
                     static_in.copy_(x, non_blocking=True)
                 graph.replay()
                 snr = static_snr.clone()
+            if world > 1:
+                mine.append(snr.unsqueeze(1))
+                continue
             acc_t = snr if count == 0 else acc_t + snr                     # noqa: F821 (defined on the first iteration)
             count += 1
+    except Exception as e:
+        if world == 1: raise
+        failed = e
     finally:
         executor.restore_quantize_state()
+    if world > 1:
+        snrs = _gather_in_batch_order(mine, len(names), torch.float32, failed, group, fn)
+        # the single-process sum, in its order and on its device (CUDA divides by a host scalar through its reciprocal, the host does not)
+        for snr in ([] if snrs is None else snrs[:, :, 0].to(next(executor.model.parameters()).device).unbind(1)):
+            acc_t = snr if count == 0 else acc_t + snr
+            count += 1
     if count == 0: return {n: 0.0 for n in names}
     vals = (acc_t / count).tolist()
     del acc
@@ -766,7 +827,7 @@ def graphwise_error_analyse(executor: TorchExecutor, batches, to_device=None, gr
 
 @torch.no_grad()
 def layerwise_error_analyse(executor: TorchExecutor, batches, interested_outputs=None, method: str = 'snr', steps: int = 8,
-                            to_device=None) -> Dict[str, float]:
+                            to_device=None, group=None) -> Dict[str, float]:
     """Which operation causes the quantisation error (ppq/quantization/analyse/layerwise.py:15-134): for every computing operation (Conv, Gemm,
     ConvTranspose, MatMul, in executor order), the error of the interested outputs when that operation alone is quantised -- its configs with
     their stored states and its baked weight, every other config FP32 (TorchExecutor.quantize_only) -- against the fp32 network.
@@ -781,11 +842,19 @@ def layerwise_error_analyse(executor: TorchExecutor, batches, interested_outputs
     (deterministic cuDNN).  Each quantised forward's outputs go to one Multi_Paired_Moments launch; the per-sample measures and batch means
     are fp64 on the device, and one copy to the host at the end feeds the running means.  The measure is the value in exact arithmetic
     rounded once per fp64 addition, where the reference sums in fp32 (fp16 / bf16 outputs: their exact upcasts) -- DESIGN.md §2.
-    Every config's state, scale and offset and every weight are as before the call, also when a batch raises."""
+    Every config's state, scale and offset and every weight are as before the call, also when a batch raises.
+    group: a torch.distributed process group of R > 1 ranks shards the batches -- `batches` is a sequence, the same on every rank, and rank r
+    measures global batches r, r + R, ... of its first min(len(batches), steps + 1); the per-batch [K, outputs] blocks and the outputs'
+    shape[0] are gathered in global batch order before the running means, so every rank returns the single-process report (bit for bit with a
+    deterministic forward on one GPU model: DESIGN.md §6).  A batch that raises on one rank makes every rank raise.  group=None runs every
+    batch here and never calls torch.distributed."""
     import itertools
 
     from .measure import MEASURES, batch_measures
+    fn = 'layerwise_error_analyse'
     if method not in MEASURES: raise ValueError(f"Unsupported measurement {method!r}: 'snr', 'mse' and 'cosine' are supported")
+    world = _analysis_world(group)
+    mine = _my_batches(batches, steps + 1, group, fn) if world > 1 else itertools.islice(batches, steps + 1)   # read once: a one-shot iterator is enough
     names = [n for n, op in executor.quantable_operations() if op.kind in COMPUTING_OP]
     if isinstance(interested_outputs, str): interested_outputs = [interested_outputs]
     if interested_outputs is not None:
@@ -809,9 +878,10 @@ def layerwise_error_analyse(executor: TorchExecutor, batches, interested_outputs
 
     dev = next(executor.model.parameters()).device
     res, weights = [], []                                                 # per batch: [K, outputs] fp64 on the device
+    failed = None
     executor.dequantize()
     try:
-        for x in itertools.islice(batches, steps + 1):                   # read once: a one-shot iterator is enough
+        for x in mine:
             if to_device is not None: x = x.to(dev, non_blocking=True) if isinstance(to_device, str) else to_device(x)
             real = run(x)
             res.append(torch.empty(len(names), len(real), dtype=torch.float64, device=dev))
@@ -822,9 +892,17 @@ def layerwise_error_analyse(executor: TorchExecutor, batches, interested_outputs
                 executor.quantize_only(None)
                 batch_measures(pred, real, method, out=res[-1][k])
             del real
+    except Exception as e:
+        if world == 1: raise
+        failed = e
     finally:
         if executor._dequantized is not None: executor.quantize_only(None)
         executor.restore_quantize_state()
+    if world > 1:                                                         # one block per batch: its [K, outputs] measures over its shape[0] row
+        blocks = [torch.cat([r, torch.tensor([w], dtype=torch.float64, device=dev)]) for r, w in zip(res, weights)] if failed is None else []
+        got = _gather_in_batch_order(blocks, len(names) + 1, torch.float64, failed, group, fn)
+        res = [] if got is None else list(got[:-1].unbind(1))
+        weights = [] if got is None else [[int(w) for w in row] for row in got[-1].tolist()]
     results = {n: 0.0 for n in names}
     if not weights: return results
     vals = torch.stack(res).cpu().tolist()                                # [batches, K, outputs]
