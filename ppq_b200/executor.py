@@ -25,6 +25,22 @@ non-quantable operation), except: a view of a known tensor shares its producer's
 passive operations upstream), and a Relu / Clip fed by an invisible operation fuses with it (refine.py:293-306).  Use the
 `Add` / `Concat` modules of this file when element-wise ops must be quantised and aligned like the reference's graph.
 
+Transformer blocks (pinned on a post-LN BERT block: tests/golden/graph_pipeline_encoder.npz, tests/test_cpu_encoder_parity.py,
+tests/test_gpu_encoder.py).  Attention written with torch.matmul and .view / .transpose is invisible to module hooks, so the opt-in modules
+`MatMul`, `Reshape`, `Transpose` and `LayerNorm` of this file stand for the reference's operators; a plain nn.LayerNorm or torch.matmul keeps
+the configs it had before they existed.  The rules, as the reference's TRT_INT8 quantizer, dispatcher and passes apply them:
+  * MatMul with two activation inputs: TensorRTQuantizer.py:50-59 makes input 1 a per-channel weight only when it is a parameter, so both
+    inputs keep per-tensor activation configs (QuantizeSimplifyPass overlaps them with their producers' outputs) and there is no weight
+    config.  It is a computing operation: it fuses with a following activation like Gemm, and layerwise_error_analyse measures it;
+  * Reshape: the constant shape input gets an FP32 config (never observed) and the conservative dispatcher leaves the operation on the INT8
+    platform (no Shape generator upstream of it); Reshape and Transpose are passive, their output shares input 0's config;
+  * LayerNormalization: gamma and beta get FP32 configs (TensorRTQuantizer.py:65-68), input 0 is overlapped with its producer's output, the
+    output is observed; no fusion, no alignment;
+  * the forwards match bit for bit on the CPU: upstream Gelu is F.gelu(x), the erf form that nn.GELU() runs (an nn.GELU(approximate='tanh')
+    is still mapped to 'Gelu' but computes a different function than the reference's operator); LayerNormalization is
+    F.layer_norm(x, gamma.shape, gamma, beta, epsilon) over the last axis, as nn.LayerNorm; Softmax is F.softmax(x, axis), as nn.Softmax;
+  * a graph input read by several operations (Q / K / V and the residual Add) gets one config per reader, each observed, as upstream.
+
 H100-native addition: `collect=True` makes the executor hand the observed fp32 tensors of a whole forward to an ArenaCalibrator
 (one multi-tensor launch per phase) instead of firing one observer launch per tensor.
 """
@@ -52,13 +68,49 @@ class Concat(torch.nn.Module):
         return torch.cat(tensors, dim=self.dim)
 
 
+class MatMul(torch.nn.Module):
+    """Product of two activations (attention's Q Kᵀ and P V) as a module, the reference's `MatMul` with no parameter input: a computing
+    operation whose two inputs and output get activation configs and which has no weight config."""
+
+    def forward(self, a, b):
+        return torch.matmul(a, b)
+
+
+class Reshape(torch.nn.Module):
+    """`x.reshape(shape)` as a module (ONNX `Reshape` with a constant shape): a passive operation, its output shares its input's config."""
+
+    def __init__(self, shape):
+        super().__init__()
+        self.shape = tuple(shape)
+
+    def forward(self, x):
+        return x.reshape(self.shape)
+
+
+class Transpose(torch.nn.Module):
+    """`x.permute(perm)` as a module (ONNX `Transpose`): a passive operation, its output shares its input's config."""
+
+    def __init__(self, perm):
+        super().__init__()
+        self.perm = tuple(perm)
+
+    def forward(self, x):
+        return x.permute(self.perm)
+
+
+class LayerNorm(torch.nn.LayerNorm):
+    """torch.nn.LayerNorm as the reference's `LayerNormalization`: input 0 and the output get activation configs, gamma and beta stay FP32
+    (TensorRTQuantizer.py:65-68), so the operation has no weight config.  A plain nn.LayerNorm stays invisible to the executor."""
+
+
 _KINDS = {torch.nn.Conv2d: 'Conv', torch.nn.ConvTranspose2d: 'ConvTranspose', torch.nn.Linear: 'Gemm', torch.nn.ReLU: 'Relu',
           torch.nn.ReLU6: 'Clip', torch.nn.MaxPool2d: 'MaxPool', torch.nn.AdaptiveAvgPool2d: 'GlobalAveragePool',
           torch.nn.AvgPool2d: 'AveragePool', torch.nn.Flatten: 'Flatten', torch.nn.Sigmoid: 'Sigmoid', torch.nn.GELU: 'Gelu',
           torch.nn.Hardswish: 'HardSwish', torch.nn.Softmax: 'Softmax', torch.nn.LeakyReLU: 'LeakyRelu', Add: 'Add', Concat: 'Concat',
           # x * sigmoid(x) as ONE module: fuses with its convolution exactly like the Conv - Sigmoid - Mul pattern upstream (refine.py:210-239),
           # where only the Mul's output keeps a live config
-          torch.nn.SiLU: 'Swish', torch.nn.Upsample: 'Resize'}
+          torch.nn.SiLU: 'Swish', torch.nn.Upsample: 'Resize',
+          MatMul: 'MatMul', Reshape: 'Reshape', Transpose: 'Transpose', LayerNorm: 'LayerNormalization'}
 
 
 def kind_of(module: torch.nn.Module) -> Optional[str]:
