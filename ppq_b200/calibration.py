@@ -161,15 +161,22 @@ class ArenaCalibrator:
     histogram of both two-phase methods is symmetric (|x| binned from 0), so asymmetric 'kl' / 'mse' are refused, as are more than
     ARENA_MAX_HIST_BINS bins.
     half_inputs=True also takes fp16 / bf16 tensors (the *_Half table kernels: the same statistics, bit for bit, as on x.float()); the
-    tensors of one `observe` call may mix element types and are served by one launch per type present."""
+    tensors of one `observe` call may mix element types and are served by one launch per type present.
+    max_batches (percentile only) makes the per-batch rows static, for a forward captured into a CUDA graph: one [max_batches, T, 2] buffer
+    and a device int64 batch counter replace the growing list.  The forward writes its quantiles into one static [T, 2] staging row,
+    observe_one selects through the slot's guess row (Quantile_T_Guess: exact, one pass when the previous batch's thresholds still hold), and
+    end_batch() files the staging row as row `counter` with one scatter and advances the counter.  begin_batch() raises before a batch
+    that would overrun the buffer."""
 
     def __init__(self, num_tensors: int, device, bins: int = None, num_of_bits: int = 8,
                  quant_min: int = -128, quant_max: int = 127, power_of_2: bool = False, min_scale: float = OBSERVER_MIN_SCALE,
                  method: str = 'kl', group=None, percentile: float = OBSERVER_PERCENTILE, select_cap: int = 1 << 16,
-                 symmetrical: bool = True, half_inputs: bool = False):
+                 symmetrical: bool = True, half_inputs: bool = False, max_batches: Optional[int] = None):
         from .ffi import extension
         if method not in ('kl', 'minmax', 'mse', 'percentile'):
             raise ValueError(f"ArenaCalibrator: unknown observer algorithm {method!r} (expected 'kl', 'minmax', 'mse' or 'percentile')")
+        if max_batches is not None and (method != 'percentile' or max_batches < 0):
+            raise ValueError(f'ArenaCalibrator: max_batches={max_batches} (static per-batch rows serve the percentile observer, >= 0 batches)')
         if method == 'kl' and not symmetrical:
             raise PermissionError('KL observer is not designed for ASYMMETRICAL quantization')
         if method == 'mse' and not symmetrical:
@@ -191,6 +198,12 @@ class ArenaCalibrator:
         self.scale = self.offset = self.best_bin_range = None
         self._stager = shared_stager(self.device, 3)
         self._pct: List[torch.Tensor] = []                               # per batch: [T, 2] {upper, lower} quantiles
+        self._rows = self._staging = self._count = None
+        if max_batches is not None:
+            self._rows = torch.zeros(max_batches, num_tensors, 2, dtype=torch.float32, device=self.device)
+            self._staging = torch.zeros(num_tensors, 2, dtype=torch.float32, device=self.device)
+            self._count = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self._begun = 0                                                  # batches begun on the host: guards the static rows
         self._select_ws = None
         # per-slot thresholds remembered from the previous batch: consecutive batches of one activation are selected in ONE pass over the tensor
         self._select_guess = self.ext.Quantile_Guess_Init(num_tensors, self.minmax) if (method == 'percentile' and self.device.type == 'cuda') else None
@@ -202,6 +215,8 @@ class ArenaCalibrator:
         self.minmax[:, 0] = float('inf'); self.minmax[:, 1] = float('-inf')
         self.hist.zero_()
         self._pct = []
+        if self._count is not None: self._count.zero_()
+        self._begun = 0
         self.phase = 1
 
     def _descs(self, tensors: Sequence[torch.Tensor], slots: Optional[Sequence[int]] = None):
@@ -218,10 +233,34 @@ class ArenaCalibrator:
     def begin_batch(self):
         """Call before every forward: the percentile observer keeps one {upper, lower} row per batch (range.py:349), whatever number of
         launches the forward's tensors are observed with."""
-        if self.method == 'percentile':
+        if self.method == 'percentile' and self._rows is not None:
+            if self._begun >= self._rows.shape[0]:
+                raise RuntimeError(f'ArenaCalibrator: batch {self._begun + 1} overruns the {self._rows.shape[0]} per-batch rows allocated '
+                                   'for a captured forward (max_batches)')
+            self._begun += 1
+        elif self.method == 'percentile':
             self._pct.append(torch.zeros(self.T, 2, dtype=torch.float32, device=self.device))
 
+    def end_batch(self):
+        """Call after every forward when the rows are static (max_batches; inside the captured graph): the staging row becomes row `counter`
+        through one device-indexed scatter, then the counter advances.  No host value is read, so every replay files its own row."""
+        if self._rows is None: return
+        self._rows.index_copy_(0, self._count, self._staging[None])
+        self._count.add_(1)
+
+    def replay_state(self) -> List[torch.Tensor]:
+        """The device buffers a forward updates in place: a warm-up forward run before a capture must leave them as it found them."""
+        return [t for t in (self.minmax, self.hist, self._select_guess if self._rows is not None else None, self._count) if t is not None]
+
+    def batch_rows(self) -> torch.Tensor:
+        """Percentile: [T, batches, 2] {upper, lower} quantiles of this rank's batches, in batch order (static rows: the first `counter`)."""
+        if self._rows is not None:
+            return self._rows[:int(self._count.item())].transpose(0, 1).contiguous()
+        if not self._pct: return torch.zeros(self.T, 0, 2, dtype=torch.float32, device=self.device)
+        return torch.stack(self._pct, dim=1)
+
     def _batch_quantiles(self) -> torch.Tensor:
+        if self._staging is not None: return self._staging
         if not self._pct: self.begin_batch()
         return self._pct[-1]
 
@@ -254,8 +293,11 @@ class ArenaCalibrator:
         """Immediate single-tensor collection into slot `index` (used while a forward is running: later in-place ops of the
         network may overwrite the tensor, so it cannot wait for the end-of-forward multi-tensor launch)."""
         if self.method == 'percentile':
-            quantile = self.ext.Quantile_T if tensor.dtype == torch.float32 else self.ext.Quantile_T_Half
-            self._batch_quantiles()[index].copy_(quantile(tensor, self.percentile))
+            if self._rows is not None:
+                self._staging[index].copy_(self.ext.Quantile_T_Guess(tensor, self.percentile, self._select_guess[index]))
+            else:
+                quantile = self.ext.Quantile_T if tensor.dtype == torch.float32 else self.ext.Quantile_T_Half
+                self._batch_quantiles()[index].copy_(quantile(tensor, self.percentile))
             self.launches += 5
             return
         if self.phase == 1:
@@ -287,8 +329,8 @@ class ArenaCalibrator:
         """Exchange + render of the finished phase.  Returns True when calibration is complete."""
         sym = self.symmetrical
         if self.method == 'percentile':
-            if not self._pct: raise ValueError('Can not render quantization config yet, Observer data collator is empty.')
-            rows = torch.stack(self._pct, dim=1)                         # [T, batches, 2]
+            rows = self.batch_rows()                                     # [T, batches, 2]
+            if rows.shape[1] == 0: raise ValueError('Can not render quantization config yet, Observer data collator is empty.')
             if self._distributed():
                 with self._timed_exchange('percentile'):
                     rows = gather_in_sample_order(rows, self.group)

@@ -641,9 +641,12 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
     deferred='auto' (default) finds out during the first forward which observed tensors the network later overwrites in place
     (torchvision adds residuals with `out += identity`), observes those immediately and everything else in one multi-tensor launch;
     graphs=True captures one forward per phase -- network kernels, per-forward weight fake-quant and the collectors -- into a CUDA
-    graph and replays it for every batch (fixed batch shape).  Capture + instantiate
-    costs more than it saves at 8-16 batches per phase, so it is off by default; it pays off for long
-    calibration sets or when the same graph is reused across calls.
+    graph and replays it for every batch, for all four methods.  It needs a fixed batch shape and the same set of observed tensors on every
+    forward; it observes tensor by tensor and ignores `deferred`.  The percentile observer's per-batch rows are then one [len(batches), T, 2]
+    device buffer, filed by a device batch counter at the end of each replay (ArenaCalibrator max_batches), so the scales are bit for bit
+    those of graphs=False.  Capture + instantiate costs more than it saves at 8-16 batches per phase for kl / minmax / mse, so it is off by
+    default; it pays off for long calibration sets or when the same graph is reused across calls.  Percentile replays are slower than the
+    eager flow's one multi-tensor select per forward, since the captured forward selects tensor by tensor (README: 1.1-2.1x on an H100).
     The observed configs must agree in range, bits, symmetry, power-of-two, minimum scale and bin / percentile overrides and be per-tensor
     (`arena_settings`); asymmetric 'kl' raises PermissionError as upstream, asymmetric 'mse' and more than 12287 KL bins raise ValueError --
     all before the first batch.
@@ -660,9 +663,13 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
                         'calibrate it with RuntimeCalibrationPass (per-observer collectors, which take fp16 / bf16).')
     from .calibration import ArenaCalibrator, is_dense
     cfgs = executor.observed_configs()
-    if graphs and method == 'percentile': raise ValueError('graphs=True needs static statistics buffers; the percentile observer keeps one row per batch')
     dev = next(executor.model.parameters()).device
-    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group, half_inputs=half_inputs, **arena_settings(cfgs, method))
+    static_rows = None
+    if graphs and method == 'percentile':                                 # the replayed per-batch rows are allocated before the first batch
+        if iter(batches) is batches or not hasattr(batches, '__len__'): batches = list(batches)
+        static_rows = len(batches)
+    cal = ArenaCalibrator(len(cfgs), dev, method=method, group=group, half_inputs=half_inputs, max_batches=static_rows,
+                          **arena_settings(cfgs, method))
     for c in cfgs: c.observer_algorithm = method
     if iter(batches) is batches: batches = list(batches)                  # a one-shot iterator would leave phase 2 without data
     static_in = None
@@ -683,18 +690,22 @@ def calibrate_arena(executor: TorchExecutor, batches, method: str = 'kl', group=
                 static_in.copy_(x, non_blocking=True)
                 if graph is None:
                     # eager run on a side stream first (cuDNN autotuning, lazy initialisation), statistics restored afterwards:
-                    # min/max are idempotent under re-observation, histogram counts are not
-                    keep_mm, keep_h = cal.minmax.clone(), cal.hist.clone()
+                    # min/max are idempotent under re-observation, histogram counts are not, the percentile batch counter would count
+                    # the warm-up batch and its select guesses would make the first replay start warm
+                    state = cal.replay_state()
+                    keep = [t.clone() for t in state]
                     side = torch.cuda.Stream(device=dev)
                     side.wait_stream(torch.cuda.current_stream(dev))
                     with torch.cuda.stream(side):
                         executor.forward(static_in, sink=cal.observe_one)
+                        cal.end_batch()
                     torch.cuda.current_stream(dev).wait_stream(side)
-                    cal.minmax.copy_(keep_mm); cal.hist.copy_(keep_h)
+                    for t, k in zip(state, keep): t.copy_(k)
                     graph = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(graph):
                         executor.forward(static_in, sink=cal.observe_one)
-                    cal.minmax.copy_(keep_mm); cal.hist.copy_(keep_h)      # capture does not execute, but stay safe
+                        cal.end_batch()
+                    for t, k in zip(state, keep): t.copy_(k)              # capture does not execute, but stay safe
                 graph.replay()
                 continue
             if to_device is not None and not overlapped: x = x.to(dev, non_blocking=True) if isinstance(to_device, str) else to_device(x)
